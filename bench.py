@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py — training scans/sec of the mv-3ddet hot path (BASELINE.json config C2: ResNet-50/16 + MinkResNet34,
-20 views 480x640, 100k points, bf16) on N B200s of one node, data-parallel over scans.
+20 views 480x640, 100k points, bf16) on N H100s of one node, data-parallel over scans.
 
   python bench.py --gpus 1 --steps K --warmup W            (N>1: launched by torch.distributed.run, one rank per GPU)
   python bench.py --impl reference ...                      (the CPU port of the reference path on the host cores)
@@ -75,6 +75,9 @@ def parse():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-e2e', action='store_true')
     ap.add_argument('--torch-profile', default='', help='write a torch.profiler kernel table of 2 steps to this path')
+    ap.add_argument('--dump-outputs', default='', metavar='DIR',
+                    help='after the timed steps, write what the last timed step computed to DIR/<name>.npy: its loss '
+                         'values and a fixed, seeded sample of the updated parameters')
     ap.add_argument('--row-order', default=None, choices=['input', 'morton'],
                     help='row order of the sparse tensors (default: ESB200_ROW_ORDER or input); morton = Z-ordered rows')
     args = ap.parse_args()
@@ -89,7 +92,23 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'fallback (H100 SXM data sheet: 3.35 TB/s HBM3)'
+
+
+def dump_outputs(path, logs, flat, n_sample=1 << 22):
+    """What the timed path hands its caller after the last timed step: the log dict of train_step (one float64 scalar per
+    loss term) and the parameters the optimiser step wrote, as a fixed, seeded sample of the flat fp32 arena (16 MB at most).
+    Inputs and initial weights are seeded and the step itself is deterministic (no order-dependent float reductions), so
+    two runs with the same arguments write identical files and two builds can be compared file by file."""
+    import re
+
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    for k, v in logs.items():
+        np.save(os.path.join(path, re.sub(r'[^A-Za-z0-9_.-]', '_', k) + '.npy'), np.asarray(float(v), dtype=np.float64))
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randint(0, flat.numel(), (min(n_sample, flat.numel()), ), generator=g).sort().values
+    np.save(os.path.join(path, 'params_sample.npy'), flat.detach()[idx.to(flat.device)].float().cpu().numpy())
 
 
 class ClockSampler:
@@ -408,6 +427,9 @@ def main():
     ms_total = float(ms)
     launches = _ffi.launch_counter['kernels']
     value = world * args.batch * args.steps / (ms_total / 1000.0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, logs, optim.arena.flat)
+        log(f'outputs of the last timed step written to {args.dump_outputs}')
 
 
     # roofline of the sparse-conv kernels from the events recorded above. Pair model (SURVEY §8d, the contract number):
@@ -439,16 +461,8 @@ def main():
     peak, peak_src = peaks()
     achieved = tot_bytes / (tot_ms / 1000.0) / 1e9 if tot_ms > 0 else 0.0
     agg = (tot_bytes + wg_bytes) / ((tot_ms + wg_ms) / 1000.0) / 1e9 if tot_ms + wg_ms > 0 else 0.0
-    traffic, traffic_note = None, None
-    for name in ('r2_traffic.json', 'r1_traffic.json'):
-        tpath = os.path.join(ROOT, 'profiles', name)
-        if os.path.exists(tpath):
-            tj = json.load(open(tpath)).get('spconv_tc_fwd_kernel')
-            if tj:
-                traffic, traffic_note = tj['dram_bytes_per_launch_avg'], tj['source']
-                break
-    roofline = {'bound': 'hbm', 'kernel': 'spconv_tc_fwd_kernel (tcgen05; forward + dgrad launches)', 'achieved': achieved,
-                'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak, 'traffic': traffic, 'traffic_note': traffic_note,
+    roofline = {'bound': 'hbm', 'kernel': 'spconv_tc_fwd_kernel (wgmma; forward + dgrad launches)', 'achieved': achieved,
+                'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak,
                 'algorithmic_bytes_per_launch_avg': tot_bytes / max(n_rec, 1), 'peak_source': peak_src,
                 'launches_timed': n_rec, 'avg_launch_us': 1000.0 * tot_ms / max(n_rec, 1),
                 'achieved_tflops': tot_flops / (tot_ms / 1000.0) / 1e12 if tot_ms > 0 else 0.0,
@@ -462,7 +476,7 @@ def main():
                 'compulsory_frac': (tot_comp / (tot_ms / 1000.0) / 1e9 / peak) if tot_ms > 0 else 0.0,
                 'compulsory_note': 'same launches and times, bytes = every input / output row and the filter moved once '
                                    '(N_in*Cin*e + N_out*Cout*e + K*Cin*Cout*e): the gather re-reads of the pair model are '
-                                   'served by the 126 MB L2, so this is the fraction of HBM peak the kernel needs',
+                                   'served by the 50 MB L2, so this is the fraction of HBM peak the kernel needs',
                 'measured': 'separate pass over the same K steps with per-launch CUDA events, 2D/3D stream overlap off so each '
                             'kernel is timed alone on the device (excluded from value)'}
 
@@ -507,7 +521,7 @@ def main():
                                   f'{args.height}x{args.width} RGB-D, {args.points} points/scan, {V["model"]}, AdamW + clip',
                       'global_batch': world * args.batch, 'parallelism': f'dp{world}',
                       'row_order': os.environ.get('ESB200_ROW_ORDER', 'input'), 'run_ahead': args.run_ahead,
-                      'l2': 'per-step working set (340 MB fp32 weights + multi-GB activations) exceeds the 126 MB L2; '
+                      'l2': 'per-step working set (340 MB fp32 weights + multi-GB activations) exceeds the 50 MB L2; '
                             f'{n_distinct} distinct input batches alternate; {n_distinct} untimed setup steps precede the W warm-up steps',
                       'loss': {k: float(v) for k, v in logs.items()}},
            'clocks': sampler.summary(), 'gpu_launches': launches, 'roofline': roofline, 'impl': 'esb200'}

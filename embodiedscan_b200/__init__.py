@@ -1,7 +1,7 @@
-"""esb200 — B200-native implementation of the EmbodiedScan multi-view 3D perception hot path.
+"""esb200 — H100-native implementation of the EmbodiedScan multi-view 3D perception hot path.
 
 Host side mirrors the reference's registry / module interface; every hot operator runs in ``libesb200.so``
-(hand-written sm_100a CUDA behind the C ABI of ``include/esb200.h``). There is no CPU fallback.
+(hand-written sm_90a CUDA behind the C ABI of ``include/esb200.h``). There is no CPU fallback.
 """
 from .registry import MODELS, TASK_UTILS  # noqa: F401
 from . import sparse  # noqa: F401

@@ -32,8 +32,6 @@ SIGNATURES = {
     'esb_kmap_tile_masks': ('piqpp', 'i'),
     'esb_spconv_tc_fwd': ('pppppqiiiip', 'i'),
     'esb_spconv_tc_wgrad': ('ppppppqiiip', 'i'),
-    'esb_spconv_tma_fwd': ('pppppqqiiiip', 'i'),
-    'esb_spconv_tma_wgrad': ('ppppppqqqiiip', 'i'),
     'esb_maxpool_fwd': ('ppppqiiip', 'i'),
     'esb_maxpool_bwd': ('pppqiip', 'i'),
     'esb_norm_fwd': ('ppppiqiippfppfipppip', 'i'),

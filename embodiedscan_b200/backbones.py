@@ -122,7 +122,7 @@ class _BiasResAct(torch.autograd.Function):
 
 
 def conv2d_tc(x: torch.Tensor, w_ohwi: torch.Tensor, bias, res, relu: bool, kh: int, kw: int, stride: int, pad: int):
-    """The folded conv + bias + residual + ReLU block in ONE tcgen05 implicit-GEMM launch with a cp.async gather
+    """The folded conv + bias + residual + ReLU block in ONE wgmma implicit-GEMM launch with a cp.async gather
     (csrc/conv2d_tc.cu: the measured baseline of csrc/conv_tma.cu). x (N,Cin,H,W) bf16 in channels_last memory; w_ohwi (Cout, r_pad) bf16 from
     :func:`pack_ohwi`; bias (Cout,) fp32 or None; res like the output or None. Forward only (frozen / inference)."""
     from . import _ffi
@@ -153,7 +153,7 @@ def tma_channels_ok(c: int) -> bool:
 
 
 def conv2d_tma(x: torch.Tensor, w_ohwi: torch.Tensor, bias, res, relu: bool, stride: int, pad: int) -> torch.Tensor:
-    """conv + bias + residual + ReLU in ONE persistent TMA + tcgen05 launch (csrc/conv_tma.cu). x (N,Cin,H,W) bf16 in
+    """conv + bias + residual + ReLU in ONE persistent TMA + wgmma launch (csrc/conv_tma.cu). x (N,Cin,H,W) bf16 in
     channels_last memory; w_ohwi (Cout,kh,kw,Cin) bf16 from :func:`ohwi`; bias (Cout,) fp32 or None; res like the output."""
     from . import _ffi
     assert x.is_cuda and x.dtype == torch.bfloat16 and x.is_contiguous(memory_format=torch.channels_last)
@@ -230,7 +230,7 @@ def conv2d_tc_dgrad(dy: torch.Tensor, w: torch.Tensor, in_hw, stride: int, pad: 
 
 def conv2d_tc_wgrad(x: torch.Tensor, dy: torch.Tensor, w_shape, stride: int, pad: int) -> torch.Tensor:
     """dL/dw of ``F.conv2d(x, w, stride, pad)``; x (N,Cin,H,W), dy (N,Cout,Ho,Wo) bf16 channels_last ->
-    (Cout,Cin,kh,kw) fp32 (split-K partial sums accumulate through fp32 atomics)."""
+    (Cout,Cin,kh,kw) fp32 (split-K partial sums are added in a fixed order: the same bits on every run)."""
     from . import _ffi
     cout, cin, kh, kw = w_shape
     assert x.dtype == dy.dtype == torch.bfloat16 and x.is_contiguous(memory_format=torch.channels_last) \
@@ -243,8 +243,8 @@ def conv2d_tc_wgrad(x: torch.Tensor, dy: torch.Tensor, w_shape, stride: int, pad
 
 class _ConvBlock2D(torch.autograd.Function):
     """out = act(conv2d(x, w) + bias + res) of the image backbone on the library's own kernels, all three passes:
-      bf16, tensor-core channel counts -> csrc/conv_tma.cu (TMA + tcgen05; fused epilogue), its stride-1 dgrad, the
-                                         transposed-gather dgrad of csrc/conv2d_tc.cu for stride 2, tcgen05 split-K wgrad
+      bf16, tensor-core channel counts -> csrc/conv_tma.cu (TMA + wgmma; fused epilogue), its stride-1 dgrad, the
+                                         transposed-gather dgrad of csrc/conv2d_tc.cu for stride 2, wgmma split-K wgrad
       fp32 (the parity arithmetic) / the 3-channel stem -> csrc/conv2d_direct.cu (fp32 FMA)
     x channels_last; w (Cout,Cin,kh,kw) in channels_last memory (= OHWI); bias fp32 (Cout,) constant; res like the output."""
 
@@ -261,7 +261,7 @@ class _ConvBlock2D(torch.autograd.Function):
                 and bias is not None and (W * 3) % 2 == 0)
         if tma:
             y = conv2d_tma(x, w_ohwi, bias, res, relu, stride, pad)
-        elif stem:       # tcgen05 with the im2col rows built in shared memory (csrc/conv_tma.cu::stem7x7_tc_kernel)
+        elif stem:       # wgmma with the im2col rows built in shared memory (csrc/conv_tma.cu::stem7x7_tc_kernel)
             Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
             y = torch.empty((N, cout, Ho, Wo), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
             _ffi.call('esb_stem7x7_tc', x.data_ptr(), w_ohwi.data_ptr(), bias.data_ptr(), y.data_ptr(), N, H, W,

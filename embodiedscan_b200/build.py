@@ -1,4 +1,4 @@
-"""Compile embodiedscan_b200/csrc/*.cu into the in-tree C-ABI library ``libesb200.so`` for sm_100a.
+"""Compile embodiedscan_b200/csrc/*.cu into the in-tree C-ABI library ``libesb200.so`` for sm_90a (H100).
 
 nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box with the snapshot.
 """
@@ -13,7 +13,7 @@ LIB = os.path.join(HERE, 'libesb200.so')
 OBJ_DIR = os.path.join(HERE, 'csrc', '_obj')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC',
+    '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC',
     '--expt-relaxed-constexpr', '-Xptxas', '-v'
 ]
 
@@ -55,7 +55,7 @@ def build_library(force=False, verbose=False):
             if log:
                 sys.stderr.write(log)
     if force or _stale(LIB, objs):
-        cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart']
+        cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a', '-lcudart']
         p = subprocess.run(cmd, capture_output=True, text=True)
         if p.returncode != 0:
             raise RuntimeError(f'link failed:\n{p.stdout}\n{p.stderr}')

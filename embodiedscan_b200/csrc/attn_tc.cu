@@ -1,15 +1,17 @@
 // esb200 — multi-head attention core of the grounding decoder (SURVEY §8 row a15: text<->3D cross-attention, self-attention
 // and text cross-attention of embodiedscan/models/layers/ground_transformer/decoder.py:89-95,151-177; 8 heads of 32 channels,
-// 256 queries, up to ~3.5k keys, key padding mask) as flash-attention tiles on tcgen05 / TMEM fed by TMA, forward AND backward.
+// 256 queries, up to ~3.5k keys, key padding mask) as flash-attention tiles on wgmma fed by TMA, forward AND backward.
 //
-// forward  (one CTA = 128 queries of one (scan, head)): Q, K, V tiles arrive as 64B-swizzled TMA boxes; S = Q K^T is one
-//   tcgen05.mma pair (M=128, N=128 keys, K=32) into TMEM; 128 softmax threads (thread = query row = TMEM lane) keep the running
-//   maximum / sum in the exp2 domain, write P (bf16) as the K-major 128B-swizzled A operand; O_tile = P V is eight more MMAs
-//   with V read as the MN-major B operand (no transpose); O is rescaled in registers. Stores O (bf16) and the log-sum-exp.
-// backward (one CTA = 128 keys of one (scan, head), loop over query tiles): S^T = K Q^T and dP^T = V dO^T in TMEM, thread =
-//   key row recomputes P^T and dS^T = P^T o (dP^T - delta) * scale, stores both as K-major A tiles; dV += P^T dO and
-//   dK += dS^T Q accumulate in TMEM over all query tiles (dO, Q read MN-major); dQ_tile = dS K reads the SAME dS^T tile as the
-//   MN-major A operand and K as the MN-major B operand, and is added to dQ (fp32) with 16-byte vector atomics.
+// forward  (one CTA = 128 queries of one (scan, head)): Q, K, V tiles arrive as 64B-swizzled TMA boxes; two consumer
+//   warpgroups own 64 queries each. S = Q K^T is one wgmma pair (m64, N=128 keys, K=32) into registers; the four lanes that
+//   hold a query row keep its running maximum / sum in the exp2 domain, write P (bf16) as the K-major 128B-swizzled A operand;
+//   O_tile = P V is eight more wgmma with V read as the MN-major B operand (no transpose); O is rescaled in registers. Stores O
+//   (bf16) and the log-sum-exp.
+// backward (one CTA = 128 keys of one (scan, head), loop over query tiles): S^T = K Q^T and dP^T = V dO^T in registers of the
+//   warpgroup that owns the key rows, which recomputes P^T and dS^T = P^T o (dP^T - delta) * scale and stores both as K-major
+//   A tiles; dV += P^T dO and dK += dS^T Q accumulate in registers over all query tiles (dO, Q read MN-major);
+//   dQ_tile = dS K reads the SAME dS^T tile as the MN-major A operand and K as the MN-major B operand and is stored to this
+//   key tile's partial of dQ; the host adds the key tiles in order.
 // Layout: q (B,H,Lq,32), k / v (B,H,Lk,32) bf16 contiguous; key_pad (B,Lk) uint8, 1 = ignore; lse (B,H,Lq) natural log.
 // Roofline: tensor pipe for long key sets, launch / latency bound at decoder sizes (256 x 3.5k x 32 per head).
 #include "tc_common.cuh"
@@ -19,15 +21,20 @@ using namespace esb_tc;
 namespace {
 
 constexpr int AT_D = 32;                    // head dimension
-constexpr int AT_THREADS = 192;             // warp 0 TMA, warp 1 MMA, warps 2-5 softmax / gradient math
+constexpr int AT_CONS = 256;                // two consumer warpgroups
+constexpr int AT_THREADS = AT_CONS + 32;    // + the TMA producer warp
 constexpr float LOG2E = 1.4426950408889634f;
 
 __device__ __forceinline__ uint32_t swz128(uint32_t row, uint32_t piece) { return row * 128u + ((piece ^ (row & 7u)) << 4); }
+// byte offset of element (row, col) of a [128 rows][128 cols] bf16 tile stored as two K-major 128B-swizzled 64-column chunks
+__device__ __forceinline__ uint32_t tile_off(int row, int col) {
+  return (uint32_t)(col >> 6) * 16384u + swz128((uint32_t)row, (uint32_t)((col & 63) >> 3)) + (uint32_t)(col & 7) * 2u;
+}
 
 // ------------------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(AT_THREADS)
+__global__ void __launch_bounds__(AT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmk,
                 const __grid_constant__ CUtensorMap tmv, const unsigned char* __restrict__ key_pad,
                 __nv_bfloat16* __restrict__ o, float* __restrict__ lse, int H, int Lq, int Lk, float scale) {
@@ -38,10 +45,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__
   uint8_t* v_s = smem + 8192 * 3;             // 2 stages x 8 KB
   uint8_t* p_s = smem + 8192 * 5;             // 2 chunks x 16 KB (offset 40960: 1024-aligned)
   uint64_t* bars = (uint64_t*)(p_s + 32768);
-  uint64_t *q_full = bars, *kv_full = bars + 1, *kv_empty = bars + 3, *s_full = bars + 5, *s_free = bars + 6,
-           *p_full = bars + 7, *o_full = bars + 8;
-  uint32_t* tmem_slot = (uint32_t*)(bars + 9);
-  unsigned char* kmask_all = (unsigned char*)(tmem_slot + 1);  // 2 x 128 flags (key tiles alternate buffers)
+  uint64_t *q_full = bars, *kv_full = bars + 1, *kv_empty = bars + 3;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int bh = blockIdx.y, b = bh / H;
@@ -50,22 +54,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-    mbar_init(s_full, 1);
-    mbar_init(s_free, 128);
-    mbar_init(p_full, 128);
-    mbar_init(o_full, 1);
+    for (int s = 0; s < 2; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], AT_CONS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmq); tma_prefetch_desc(&tmk); tma_prefetch_desc(&tmv);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t t_s = tmem_base, t_o = tmem_base + 128;
 
-  if (warp == 0) {
+  if (threadIdx.x >= AT_CONS) {
     if (lane == 0) {
       mbar_expect_tx(q_full, 8192);
       tma_load_2d(&tmq, q_full, smem_u32(q_s), 0, bh * Lq + q0);
@@ -77,117 +72,95 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__
         tma_load_2d(&tmv, &kv_full[s], smem_u32(v_s + s * 8192), 0, bh * Lk + j * 128);
       }
     }
-  } else if (warp == 1) {
-    const uint32_t id_s = make_idesc(128, 128, 0, 0), id_o = make_idesc(128, AT_D, 0, 1);
-    mbar_wait(q_full, 0);
-    for (int j = 0; j < n_kt; ++j) {
-      const int s = j & 1;
-      mbar_wait(&kv_full[s], (j >> 1) & 1);
-      mbar_wait(s_free, (j & 1) ^ 1);                          // the softmax threads have read S of tile j-1 out of TMEM
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t qa = smem_u32(q_s), ka = smem_u32(k_s + s * 8192);
-#pragma unroll
-        for (int kk = 0; kk < 2; ++kk)
-          umma_bf16(t_s, make_desc_sw(qa + kk * 32, 16, 512, 4), make_desc_sw(ka + kk * 32, 16, 512, 4), id_s, kk ? 1u : 0u);
-        umma_commit(s_full);
-      }
-      __syncwarp();
-      mbar_wait(p_full, j & 1);                                // P of tile j is in shared memory, O_tile of j-1 consumed
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t pa = smem_u32(p_s), va = smem_u32(v_s + s * 8192);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)
-          umma_bf16(t_o, make_desc_sw(pa + (kk >> 2) * 16384 + (kk & 3) * 32, 16, 1024, 2),
-                    make_desc_sw(va + kk * 1024, 2048, 512, 4), id_o, kk ? 1u : 0u);
-        umma_commit(o_full);
-        umma_commit(&kv_empty[s]);
-      }
-      __syncwarp();
-    }
-    tc_fence_before();
-  } else {
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;                            // query row of the tile = TMEM lane
-    const int et = r;
-    const float sc2 = scale * LOG2E;
-    float m = -INFINITY, l = 0.f, acc[AT_D];
-#pragma unroll
-    for (int e = 0; e < AT_D; ++e) acc[e] = 0.f;
-    for (int j = 0; j < n_kt; ++j) {
-      unsigned char* kmask = kmask_all + (j & 1) * 128;
-      {   // key mask of this tile (identical for every query row)
-        const int kj = j * 128 + et;
-        kmask[et] = (kj >= Lk || (key_pad != nullptr && key_pad[(long long)b * Lk + kj])) ? 1 : 0;
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      // pass 1 over the S tile in TMEM: running maximum (TMEM reads are cheap; keeping 128 scores in registers is not)
-      float mx = m;
-#pragma unroll 1
-      for (int c0 = 0; c0 < 128; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32(t_s + ((uint32_t)(quad * 32) << 16) + (uint32_t)c0, v);
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (!kmask[c0 + i]) mx = fmaxf(mx, __uint_as_float(v[i]) * sc2);
-      }
-      const float m_use = mx == -INFINITY ? 0.f : mx;
-      const float alpha = exp2f(m - m_use);                    // m = -inf -> 0
-      float rs = 0.f;
-      // pass 2: probabilities -> bf16 A operand in shared memory
-#pragma unroll 1
-      for (int c0 = 0; c0 < 128; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32(t_s + ((uint32_t)(quad * 32) << 16) + (uint32_t)c0, v);
-        if (c0 == 96) {
-          tc_fence_before();
-          mbar_arrive(s_free);
-        }
-#pragma unroll
-        for (int pj = 0; pj < 4; ++pj) {                       // 4 pieces of 8 keys
-          uint32_t w[4];
-#pragma unroll
-          for (int h = 0; h < 4; ++h) {
-            const int i0 = pj * 8 + 2 * h;
-            const float p0 = kmask[c0 + i0] ? 0.f : exp2f(__uint_as_float(v[i0]) * sc2 - m_use);
-            const float p1 = kmask[c0 + i0 + 1] ? 0.f : exp2f(__uint_as_float(v[i0 + 1]) * sc2 - m_use);
-            rs += p0 + p1;
-            w[h] = pack_bf16(__float_as_uint(p0), __float_as_uint(p1));
-          }
-          *reinterpret_cast<uint4*>(p_s + (c0 >> 6) * 16384 + swz128((uint32_t)r, (uint32_t)(((c0 & 63) >> 3) + pj))) =
-              make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-      l = l * alpha + rs;
-      m = mx;
-      fence_proxy_async();
-      mbar_arrive(p_full);
-      mbar_wait(o_full, j & 1);
-      tc_fence_after();
-      uint32_t ov[32];
-      tmem_ld32(t_o + ((uint32_t)(quad * 32) << 16), ov);
-      tc_fence_before();
-#pragma unroll
-      for (int e = 0; e < AT_D; ++e) acc[e] = acc[e] * alpha + __uint_as_float(ov[e]);
-    }
-    if (q0 + r < Lq) {
-      const float inv = l > 0.f ? 1.f / l : 0.f;
-      uint32_t w[16];
-#pragma unroll
-      for (int h = 0; h < 16; ++h) w[h] = pack_bf16(__float_as_uint(acc[2 * h] * inv), __float_as_uint(acc[2 * h + 1] * inv));
-      uint4* dst = reinterpret_cast<uint4*>(o + ((long long)bh * Lq + q0 + r) * AT_D);
-#pragma unroll
-      for (int h = 0; h < 4; ++h) dst[h] = make_uint4(w[4 * h], w[4 * h + 1], w[4 * h + 2], w[4 * h + 3]);
-      lse[(long long)bh * Lq + q0 + r] = l > 0.f ? (m + log2f(l)) * 0.6931471805599453f : -INFINITY;
-    }
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
+  // ---- consumers: warpgroup wg owns queries 64 wg .. 64 wg + 63 of the tile; this thread holds rows ra and ra + 8 ----
+  const int wg = threadIdx.x >> 7;
+  const int ra = wg * 64 + 16 * (warp & 3) + (lane >> 2);
+  const int cq = 2 * (lane & 3);                             // first of this thread's two columns in every 8-column block
+  const float sc2 = scale * LOG2E;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};    // running maximum (exp2 domain) / this thread's partial sum
+  float acc[AT_D / 2], sacc[64], oacc[AT_D / 2];
+#pragma unroll
+  for (int e = 0; e < AT_D / 2; ++e) acc[e] = 0.f;
+  mbar_wait(q_full, 0);
+  const uint32_t qa = smem_u32(q_s) + wg * 4096, pa = smem_u32(p_s) + wg * 8192;
+  for (int j = 0; j < n_kt; ++j) {
+    const int s = j & 1;
+    mbar_wait(&kv_full[s], (j >> 1) & 1);
+    const uint32_t ka = smem_u32(k_s + s * 8192), va = smem_u32(v_s + s * 8192);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 2; ++kk)
+      wgmma_bf16<128, 0, 0>(sacc, make_desc_sw(qa + kk * 32, 16, 512, SW64), make_desc_sw(ka + kk * 32, 16, 512, SW64), kk > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence<64>(sacc);
+    // key mask of this thread's 32 columns (identical for every query row)
+    uint32_t dead = 0;
+#pragma unroll
+    for (int jb = 0; jb < 16; ++jb)
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const int kj = j * 128 + 8 * jb + cq + u;
+        if (kj >= Lk || (key_pad != nullptr && key_pad[(long long)b * Lk + kj])) dead |= 1u << (2 * jb + u);
+      }
+    float alpha[2], m_use[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = m[h];
+#pragma unroll
+      for (int jb = 0; jb < 16; ++jb)
+#pragma unroll
+        for (int u = 0; u < 2; ++u)
+          if (!((dead >> (2 * jb + u)) & 1)) mx = fmaxf(mx, sacc[4 * jb + 2 * h + u] * sc2);
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      m_use[h] = mx == -INFINITY ? 0.f : mx;
+      alpha[h] = exp2f(m[h] - m_use[h]);                     // m = -inf -> 0
+      m[h] = mx;
+    }
+    // probabilities -> bf16 A operand in shared memory (this warpgroup's rows only)
+    float rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int jb = 0; jb < 16; ++jb)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float p0 = ((dead >> (2 * jb)) & 1) ? 0.f : exp2f(sacc[4 * jb + 2 * h] * sc2 - m_use[h]);
+        const float p1 = ((dead >> (2 * jb + 1)) & 1) ? 0.f : exp2f(sacc[4 * jb + 2 * h + 1] * sc2 - m_use[h]);
+        rs[h] += p0 + p1;
+        *reinterpret_cast<uint32_t*>(p_s + tile_off(ra + 8 * h, 8 * jb + cq)) = pack_bf16(__float_as_uint(p0), __float_as_uint(p1));
+      }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l[h] = l[h] * alpha[h] + rs[h];
+    fence_proxy_async();
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // the warpgroup's P rows are complete
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+      wgmma_bf16<AT_D, 0, 1>(oacc, make_desc_sw(pa + (kk >> 2) * 16384 + (kk & 3) * 32, 16, 1024, SW128),
+                             make_desc_sw(va + kk * 1024, 2048, 512, SW64), kk > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence<AT_D / 2>(oacc);
+    if (lane == 0) mbar_arrive(&kv_empty[s]);
+#pragma unroll
+    for (int e = 0; e < AT_D / 2; ++e) acc[e] = acc[e] * alpha[(e >> 1) & 1] + oacc[e];
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+    const int qi = q0 + ra + 8 * h;
+    if (qi < Lq) {
+      const float inv = l[h] > 0.f ? 1.f / l[h] : 0.f;
+      __nv_bfloat16* dst = o + ((long long)bh * Lq + qi) * AT_D;
+#pragma unroll
+      for (int jb = 0; jb < AT_D / 8; ++jb)
+        *reinterpret_cast<uint32_t*>(dst + 8 * jb + cq) =
+            pack_bf16(__float_as_uint(acc[4 * jb + 2 * h] * inv), __float_as_uint(acc[4 * jb + 2 * h + 1] * inv));
+      if ((lane & 3) == 0) lse[(long long)bh * Lq + qi] = l[h] > 0.f ? (m[h] + log2f(l[h])) * 0.6931471805599453f : -INFINITY;
+    }
   }
 }
 
@@ -217,7 +190,7 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __n
 // ------------------------------------------------------------------------------------------------------------
 // backward
 // ------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(AT_THREADS)
+__global__ void __launch_bounds__(AT_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__ CUtensorMap tmk,
                 const __grid_constant__ CUtensorMap tmv, const __grid_constant__ CUtensorMap tmdo,
                 const unsigned char* __restrict__ key_pad, const float* __restrict__ lse, const float* __restrict__ delta,
@@ -234,9 +207,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__
   float* lse2_all = (float*)(smem + 49152 + 65536);        // 2 x 128: lse * log2e of the query tile (tiles alternate buffers)
   float* delta_all = lse2_all + 256;
   uint64_t* bars = (uint64_t*)(delta_all + 256);
-  uint64_t *kv_full = bars, *qd_full = bars + 1, *qd_empty = bars + 3, *sdp_full = bars + 5, *st_free = bars + 6,
-           *pds_full = bars + 7, *dq_full = bars + 8, *dq_free = bars + 9, *fin_full = bars + 10;
-  uint32_t* tmem_slot = (uint32_t*)(bars + 11);
+  uint64_t *kv_full = bars, *qd_full = bars + 1, *qd_empty = bars + 3;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int bh = blockIdx.y, b = bh / H;
@@ -245,24 +216,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__
 
   if (threadIdx.x == 0) {
     mbar_init(kv_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(&qd_full[s], 1); mbar_init(&qd_empty[s], 1); }
-    mbar_init(sdp_full, 1);
-    mbar_init(st_free, 128);
-    mbar_init(pds_full, 128);
-    mbar_init(dq_full, 1);
-    mbar_init(dq_free, 128);
-    mbar_init(fin_full, 1);
+    for (int s = 0; s < 2; ++s) { mbar_init(&qd_full[s], 1); mbar_init(&qd_empty[s], AT_CONS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmq); tma_prefetch_desc(&tmk); tma_prefetch_desc(&tmv); tma_prefetch_desc(&tmdo);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t t_st = tmem_base, t_dp = tmem_base + 128, t_dv = tmem_base + 256, t_dk = tmem_base + 288, t_dq = tmem_base + 320;
 
-  if (warp == 0) {
+  if (threadIdx.x >= AT_CONS) {
     if (lane == 0) {
       mbar_expect_tx(kv_full, 16384);
       tma_load_2d(&tmk, kv_full, smem_u32(k_s), 0, bh * Lk + k0);
@@ -275,138 +235,111 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmq, const __grid_constant__
         tma_load_2d(&tmdo, &qd_full[s], smem_u32(do_s + s * 8192), 0, bh * Lq + i * 128);
       }
     }
-  } else if (warp == 1) {
-    const uint32_t id_s = make_idesc(128, 128, 0, 0);          // S^T, dP^T: A, B K-major
-    const uint32_t id_g = make_idesc(128, AT_D, 0, 1);         // dV, dK: A K-major, B MN-major
-    const uint32_t id_q = make_idesc(128, AT_D, 1, 1);         // dQ: A MN-major (dS^T read transposed), B MN-major
-    mbar_wait(kv_full, 0);
-    for (int i = 0; i < n_qt; ++i) {
-      const int s = i & 1;
-      mbar_wait(&qd_full[s], (i >> 1) & 1);
-      mbar_wait(st_free, (i & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t ka = smem_u32(k_s), va = smem_u32(v_s), qa = smem_u32(q_s + s * 8192), da = smem_u32(do_s + s * 8192);
-      if (lane == 0) {
+    return;
+  }
+  // ---- consumers: warpgroup wg owns keys 64 wg .. 64 wg + 63 (S^T, dP^T, dV, dK rows) and queries 64 wg .. of every query
+  // tile (dQ rows); this thread holds fragment rows ra and ra + 8 ----
+  const int t = threadIdx.x, wg = t >> 7;
+  const int ra = wg * 64 + 16 * (warp & 3) + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  bool k_dead[2];
 #pragma unroll
-        for (int kk = 0; kk < 2; ++kk)
-          umma_bf16(t_st, make_desc_sw(ka + kk * 32, 16, 512, 4), make_desc_sw(qa + kk * 32, 16, 512, 4), id_s, kk ? 1u : 0u);
-#pragma unroll
-        for (int kk = 0; kk < 2; ++kk)
-          umma_bf16(t_dp, make_desc_sw(va + kk * 32, 16, 512, 4), make_desc_sw(da + kk * 32, 16, 512, 4), id_s, kk ? 1u : 0u);
-        umma_commit(sdp_full);
-      }
-      __syncwarp();
-      mbar_wait(pds_full, i & 1);                              // P^T and dS^T of this query tile are in shared memory
-      mbar_wait(dq_free, (i & 1) ^ 1);                         // dQ of the previous tile has been read out of TMEM
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t pa = smem_u32(pt_s), sa = smem_u32(ds_s);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {                       // reduction over the 128 queries of the tile
-          const uint32_t a_off = (kk >> 2) * 16384 + (kk & 3) * 32;
-          umma_bf16(t_dv, make_desc_sw(pa + a_off, 16, 1024, 2), make_desc_sw(da + kk * 1024, 2048, 512, 4), id_g,
-                    (i > 0 || kk > 0) ? 1u : 0u);
-          umma_bf16(t_dk, make_desc_sw(sa + a_off, 16, 1024, 2), make_desc_sw(qa + kk * 1024, 2048, 512, 4), id_g,
-                    (i > 0 || kk > 0) ? 1u : 0u);
-        }
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)                         // reduction over the 128 keys of this CTA
-          umma_bf16(t_dq, make_desc_sw(sa + kk * 2048, 16384, 1024, 2), make_desc_sw(ka + kk * 1024, 2048, 512, 4), id_q,
-                    kk ? 1u : 0u);
-        umma_commit(dq_full);
-        umma_commit(&qd_empty[s]);
-        if (i == n_qt - 1) umma_commit(fin_full);
-      }
-      __syncwarp();
+  for (int h = 0; h < 2; ++h) {
+    const int kj = k0 + ra + 8 * h;
+    k_dead[h] = kj >= Lk || (key_pad != nullptr && key_pad[(long long)b * Lk + kj]);
+  }
+  const float sc2 = scale * LOG2E;
+  float sacc[64], pacc[64], dvacc[AT_D / 2], dkacc[AT_D / 2], dqacc[AT_D / 2];
+  const uint32_t ka = smem_u32(k_s), va = smem_u32(v_s), pa = smem_u32(pt_s), sa = smem_u32(ds_s);
+  mbar_wait(kv_full, 0);
+  for (int i = 0; i < n_qt; ++i) {
+    const int s = i & 1;
+    float* lse2_s = lse2_all + (i & 1) * 128;
+    float* delta_s = delta_all + (i & 1) * 128;
+    if (t < 128) {
+      const int qi = i * 128 + t;
+      lse2_s[t] = qi < Lq ? lse[(long long)bh * Lq + qi] * LOG2E : INFINITY;     // +inf -> p = 0 for absent queries
+      delta_s[t] = qi < Lq ? delta[(long long)bh * Lq + qi] : 0.f;
     }
-    tc_fence_before();
-  } else {
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;                            // key row of this CTA (S^T lanes) / query row (dQ lanes)
-    const int kj = k0 + r;
-    const bool k_dead = kj >= Lk || (key_pad != nullptr && key_pad[(long long)b * Lk + kj]);
-    const float sc2 = scale * LOG2E;
-    for (int i = 0; i < n_qt; ++i) {
-      float* lse2_s = lse2_all + (i & 1) * 128;
-      float* delta_s = delta_all + (i & 1) * 128;
-      {
-        const int qi = i * 128 + r;
-        lse2_s[r] = qi < Lq ? lse[(long long)bh * Lq + qi] * LOG2E : INFINITY;     // +inf -> p = 0 for absent queries
-        delta_s[r] = qi < Lq ? delta[(long long)bh * Lq + qi] : 0.f;
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      mbar_wait(sdp_full, i & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < 128; c0 += 32) {
-        uint32_t sv[32], dv_[32];
-        tmem_ld32(t_st + ((uint32_t)(quad * 32) << 16) + (uint32_t)c0, sv);
-        tmem_ld32(t_dp + ((uint32_t)(quad * 32) << 16) + (uint32_t)c0, dv_);
-        if (c0 == 96) {
-          tc_fence_before();
-          mbar_arrive(st_free);
+    // lse2 / delta of this tile are written; both warpgroups are past tile i - 1 (its dQ MMA read every row of dS^T)
+    asm volatile("bar.sync 1, %0;" ::"n"(AT_CONS) : "memory");
+    mbar_wait(&qd_full[s], (i >> 1) & 1);
+    const uint32_t qa = smem_u32(q_s + s * 8192), da = smem_u32(do_s + s * 8192);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 2; ++kk)
+      wgmma_bf16<128, 0, 0>(sacc, make_desc_sw(ka + wg * 4096 + kk * 32, 16, 512, SW64), make_desc_sw(qa + kk * 32, 16, 512, SW64),
+                            kk > 0);
+#pragma unroll
+    for (int kk = 0; kk < 2; ++kk)
+      wgmma_bf16<128, 0, 0>(pacc, make_desc_sw(va + wg * 4096 + kk * 32, 16, 512, SW64), make_desc_sw(da + kk * 32, 16, 512, SW64),
+                            kk > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence<64>(sacc);
+    acc_fence<64>(pacc);
+#pragma unroll
+    for (int jb = 0; jb < 16; ++jb)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float p[2], ds[2];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int c = 8 * jb + cq + u, e = 4 * jb + 2 * h + u;
+          const float ex = k_dead[h] ? 0.f : exp2f(sacc[e] * sc2 - lse2_s[c]);
+          p[u] = ex;
+          ds[u] = ex * (pacc[e] - delta_s[c]) * scale;
         }
-#pragma unroll
-        for (int pj = 0; pj < 4; ++pj) {
-          uint32_t wp[4], wd[4];
-#pragma unroll
-          for (int h = 0; h < 4; ++h) {
-            float p[2], ds[2];
-#pragma unroll
-            for (int u = 0; u < 2; ++u) {
-              const int c = c0 + pj * 8 + 2 * h + u;
-              const float e = k_dead ? 0.f : exp2f(__uint_as_float(sv[pj * 8 + 2 * h + u]) * sc2 - lse2_s[c]);
-              p[u] = e;
-              ds[u] = e * (__uint_as_float(dv_[pj * 8 + 2 * h + u]) - delta_s[c]) * scale;
-            }
-            wp[h] = pack_bf16(__float_as_uint(p[0]), __float_as_uint(p[1]));
-            wd[h] = pack_bf16(__float_as_uint(ds[0]), __float_as_uint(ds[1]));
-          }
-          const uint32_t off = (uint32_t)(c0 >> 6) * 16384u + swz128((uint32_t)r, (uint32_t)(((c0 & 63) >> 3) + pj));
-          *reinterpret_cast<uint4*>(pt_s + off) = make_uint4(wp[0], wp[1], wp[2], wp[3]);
-          *reinterpret_cast<uint4*>(ds_s + off) = make_uint4(wd[0], wd[1], wd[2], wd[3]);
-        }
+        const uint32_t off = tile_off(ra + 8 * h, 8 * jb + cq);
+        *reinterpret_cast<uint32_t*>(pt_s + off) = pack_bf16(__float_as_uint(p[0]), __float_as_uint(p[1]));
+        *reinterpret_cast<uint32_t*>(ds_s + off) = pack_bf16(__float_as_uint(ds[0]), __float_as_uint(ds[1]));
       }
-      fence_proxy_async();
-      mbar_arrive(pds_full);
-      mbar_wait(dq_full, i & 1);
-      tc_fence_after();
-      uint32_t qv[32];
-      tmem_ld32(t_dq + ((uint32_t)(quad * 32) << 16), qv);
-      tc_fence_before();
-      mbar_arrive(dq_free);
-      const int qi = i * 128 + r;
+    fence_proxy_async();
+    asm volatile("bar.sync 1, %0;" ::"n"(AT_CONS) : "memory");   // P^T and dS^T of this query tile are complete
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {                           // reduction over the 128 queries of the tile
+      const uint32_t a_off = wg * 8192 + (kk >> 2) * 16384 + (kk & 3) * 32;
+      wgmma_bf16<AT_D, 0, 1>(dvacc, make_desc_sw(pa + a_off, 16, 1024, SW128), make_desc_sw(da + kk * 1024, 2048, 512, SW64),
+                             i > 0 || kk > 0);
+      wgmma_bf16<AT_D, 0, 1>(dkacc, make_desc_sw(sa + a_off, 16, 1024, SW128), make_desc_sw(qa + kk * 1024, 2048, 512, SW64),
+                             i > 0 || kk > 0);
+    }
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)                             // reduction over the 128 keys of this CTA
+      wgmma_bf16<AT_D, 1, 1>(dqacc, make_desc_sw(sa + wg * 16384 + kk * 2048, 16384, 1024, SW128),
+                             make_desc_sw(ka + kk * 1024, 2048, 512, SW64), kk > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence<AT_D / 2>(dvacc);
+    acc_fence<AT_D / 2>(dkacc);
+    acc_fence<AT_D / 2>(dqacc);
+    if (lane == 0) mbar_arrive(&qd_empty[s]);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int qi = i * 128 + ra + 8 * h;
       if (qi < Lq) {
-        float* dst = dq + ((long long)bh * Lq + qi) * AT_D;
+        float* dst = dq + (((long long)blockIdx.x * gridDim.y + bh) * Lq + qi) * AT_D;     // partial of key tile blockIdx.x
 #pragma unroll
-        for (int h = 0; h < 8; ++h)
-          atomicAdd(reinterpret_cast<float4*>(dst + 4 * h),
-                    make_float4(__uint_as_float(qv[4 * h]), __uint_as_float(qv[4 * h + 1]), __uint_as_float(qv[4 * h + 2]),
-                                __uint_as_float(qv[4 * h + 3])));
-      }
-    }
-    mbar_wait(fin_full, 0);
-    tc_fence_after();
-    uint32_t a[32], c[32];
-    tmem_ld32(t_dv + ((uint32_t)(quad * 32) << 16), a);
-    tmem_ld32(t_dk + ((uint32_t)(quad * 32) << 16), c);
-    tc_fence_before();
-    if (kj < Lk) {
-      uint4* pv = reinterpret_cast<uint4*>(dv + ((long long)bh * Lk + kj) * AT_D);
-      uint4* pk = reinterpret_cast<uint4*>(dk + ((long long)bh * Lk + kj) * AT_D);
-#pragma unroll
-      for (int h = 0; h < 4; ++h) {
-        pv[h] = make_uint4(pack_bf16(a[8 * h], a[8 * h + 1]), pack_bf16(a[8 * h + 2], a[8 * h + 3]), pack_bf16(a[8 * h + 4], a[8 * h + 5]),
-                           pack_bf16(a[8 * h + 6], a[8 * h + 7]));
-        pk[h] = make_uint4(pack_bf16(c[8 * h], c[8 * h + 1]), pack_bf16(c[8 * h + 2], c[8 * h + 3]), pack_bf16(c[8 * h + 4], c[8 * h + 5]),
-                           pack_bf16(c[8 * h + 6], c[8 * h + 7]));
+        for (int jb = 0; jb < AT_D / 8; ++jb)
+          *reinterpret_cast<float2*>(dst + 8 * jb + cq) = make_float2(dqacc[4 * jb + 2 * h], dqacc[4 * jb + 2 * h + 1]);
       }
     }
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int kj = k0 + ra + 8 * h;
+    if (kj < Lk) {
+      __nv_bfloat16* pv = dv + ((long long)bh * Lk + kj) * AT_D;
+      __nv_bfloat16* pk = dk + ((long long)bh * Lk + kj) * AT_D;
+#pragma unroll
+      for (int jb = 0; jb < AT_D / 8; ++jb) {
+        *reinterpret_cast<uint32_t*>(pv + 8 * jb + cq) =
+            pack_bf16(__float_as_uint(dvacc[4 * jb + 2 * h]), __float_as_uint(dvacc[4 * jb + 2 * h + 1]));
+        *reinterpret_cast<uint32_t*>(pk + 8 * jb + cq) =
+            pack_bf16(__float_as_uint(dkacc[4 * jb + 2 * h]), __float_as_uint(dkacc[4 * jb + 2 * h + 1]));
+      }
+    }
   }
 }
 
@@ -429,7 +362,7 @@ extern "C" int esb_attn_fwd(const void* q, const void* k, const void* v, const u
   if (rc == ESB_OK) rc = rows32_map(&tmk, k, (long long)B * H * Lk);
   if (rc == ESB_OK) rc = rows32_map(&tmv, v, (long long)B * H * Lk);
   if (rc != ESB_OK) return rc;
-  const size_t smem = 8192 * 5 + 32768 + 16 * 8 + 16 + 256 + 1024;
+  const size_t smem = 8192 * 5 + 32768 + 8 * 8 + 1024;
   cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { esb_set_error("esb_attn_fwd: smem attr: %s", cudaGetErrorString(e)); return ESB_ECUDA; }
   dim3 grid((Lq + 127) / 128, B * H);
@@ -438,7 +371,8 @@ extern "C" int esb_attn_fwd(const void* q, const void* k, const void* v, const u
   return ESB_OK;
 }
 
-// dq (B,H,Lq,32) fp32 ZEROED BY THE CALLER (key tiles accumulate with vector atomics); dk, dv (B,H,Lk,32) bf16 written once;
+// dq (B,H,Lq,32) fp32 += the query gradient (zeroed by the caller; the key tiles' partials are added in order); dk, dv
+// (B,H,Lk,32) bf16 written once;
 // delta (B,H,Lq) fp32 workspace.
 extern "C" int esb_attn_bwd(const void* q, const void* k, const void* v, const unsigned char* key_pad, const void* o,
                             const void* dout, const float* lse, float* delta, float* dq, void* dk, void* dv, int B, int H, int Lq,
@@ -454,12 +388,17 @@ extern "C" int esb_attn_bwd(const void* q, const void* k, const void* v, const u
   const long long rows = (long long)B * H * Lq;
   attn_delta_kernel<<<esb_div_up(rows, 256), 256, 0, stream>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)dout, delta, rows);
   ESB_CUDA_LAUNCH_CHECK("attn_delta_kernel");
-  const size_t smem = 49152 + 65536 + 2048 + 16 * 8 + 16 + 1024;
+  const size_t smem = 49152 + 65536 + 2048 + 8 * 8 + 1024;
   cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { esb_set_error("esb_attn_bwd: smem attr: %s", cudaGetErrorString(e)); return ESB_ECUDA; }
   dim3 grid((Lk + 127) / 128, B * H);
-  attn_bwd_kernel<<<grid, AT_THREADS, smem, stream>>>(tmq, tmk, tmv, tmdo, key_pad, lse, delta, dq, (__nv_bfloat16*)dk,
+  const long long width = rows * AT_D;
+  float* part = nullptr;
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, sizeof(float) * grid.x * width, stream));
+  attn_bwd_kernel<<<grid, AT_THREADS, smem, stream>>>(tmq, tmk, tmv, tmdo, key_pad, lse, delta, part, (__nv_bfloat16*)dk,
                                                       (__nv_bfloat16*)dv, H, Lq, Lk, scale);
   ESB_CUDA_LAUNCH_CHECK("attn_bwd_kernel");
-  return ESB_OK;
+  rc = esb_sum_partial_rows(part, (int)grid.x, width, dq, 1, stream);
+  ESB_CUDA_CALL(esb_scratch_free(part, stream));
+  return rc;
 }

@@ -1,5 +1,6 @@
-// esb200 — shared device/host helpers for the sm_100a kernels behind libesb200.so.
-// Nothing here allocates device memory: the caller (PyTorch host) owns every buffer.
+// esb200 — shared device/host helpers for the sm_90a kernels behind libesb200.so.
+// Buffers that cross the C ABI belong to the caller (PyTorch host); the only memory the library takes itself is the
+// stream-ordered scratch of its deterministic reductions.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -38,6 +39,17 @@ void esb_set_error(const char* fmt, ...);
 
 static inline int esb_div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline size_t esb_align(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
+// ---- deterministic reductions (scratch.cu) --------------------------------------------------------------------------
+// Kernels never combine partial sums with float atomics (their order, and so the rounding, would change from run to run):
+// each block / split writes its partial to stream-ordered scratch memory and one of the reducers below adds the partials
+// in index order. The scratch comes from the device's stream-ordered pool and is released on the same stream.
+cudaError_t esb_scratch_alloc(void** p, size_t bytes, cudaStream_t s);
+cudaError_t esb_scratch_free(void* p, cudaStream_t s);
+// out[j] (+)= sum over p = 0 .. n_parts-1 of part[p * width + j], in that order (accumulate = 0 overwrites out)
+int esb_sum_partial_rows(const float* part, int n_parts, long long width, float* out, int accumulate, cudaStream_t s);
+
+// streaming multiprocessors of the current device (grid sizing; read once per device)
+int esb_sm_count();
 
 
 // ---- coordinate key packing: [b:16 | x:16 | y:16 | z:16], xyz biased by 2^15 ----

@@ -1,7 +1,7 @@
 // esb200 — direct (SIMT, fp32-accumulate) NHWC 2D convolution, its two gradients and the stem's max pooling.
 // Two jobs on the per-view image backbone (SURVEY §8 row a5; mmdet.ResNet called at
 // embodiedscan/models/detectors/sparse_featfusion_single_stage.py:130-136):
-//   * the fp32 PARITY arithmetic of every 2D convolution (the tcgen05 kernels of conv_tma.cu / conv2d_tc.cu take bf16
+//   * the fp32 PARITY arithmetic of every 2D convolution (the wgmma kernels of conv_tma.cu / conv2d_tc.cu take bf16
 //     operands; fp32 FMA is what the 1e-3 bound of BASELINE.json is checked in), forward, dgrad and wgrad;
 //   * the 7x7/2 stem on the 3-channel image in either dtype (Cin = 3 cannot feed a 16-byte TMA box) and the 3x3/2 max pool.
 // Layouts: x (n,H,W,cin), w OHWI (cout,kh,kw,cin), y (n,Ho,Wo,cout); T = float or bf16, accumulation fp32.
@@ -240,7 +240,7 @@ extern "C" int esb_conv2d_direct_wgrad(const void* x, const void* dy, float* dw_
   const long long M = (long long)n_img * Ho * Wo;
   if (M == 0) return ESB_OK;
   const int pair_blocks = esb_div_up((long long)cin * cout, 256);
-  long long slices = (4LL * 148 * 8) / ((long long)pair_blocks * kh * kw) + 1;     // enough CTAs to fill the device
+  long long slices = (4LL * esb_sm_count() * 8) / ((long long)pair_blocks * kh * kw) + 1;   // enough CTAs to fill the device
   if (slices > 1024) slices = 1024;
   int slice = (int)((M + slices - 1) / slices);
   if (slice < 64) slice = 64;

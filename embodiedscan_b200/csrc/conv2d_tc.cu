@@ -1,10 +1,10 @@
-// esb200 — dense 2D convolution on the 5th-generation tensor cores (tcgen05 + TMEM), bf16 in / fp32 accumulate:
+// esb200 — dense 2D convolution on the Hopper tensor cores (wgmma), bf16 in / fp32 accumulate:
 // the per-view image backbone (SURVEY §8 row a5: mmdet.ResNet(depth=50, base_channels=16) called at
 // embodiedscan/models/detectors/sparse_featfusion_single_stage.py:130-136) as an implicit GEMM with the frozen
 // BatchNorm folded into the weights and bias + residual + ReLU fused into the epilogue.
 //
-// STATUS: validated on the B200 in round 2 (19/19 cases); superseded on the measured path by conv_tma.cu (TMA-fed), kept as its
-// measured cp.async baseline (wgrad: 2.5-4.5x slower than the TMA version) and as the dgrad for strides above 2.
+// STATUS: superseded on the measured path by conv_tma.cu (TMA-fed); kept as its cp.async baseline and as the dgrad for
+// strides above 2.
 //
 // GEMM view: M = n_img*Ho*Wo output pixels, N = Cout, reduction R = kh*kw*Cin ordered (ky, kx, ci) — i.e. the weight
 // in OHWI (= PyTorch channels_last) layout IS the K-major B operand, row n = output channel, R contiguous, zero padded
@@ -12,8 +12,9 @@
 // N_TILE channels and gathers, per 64-wide reduction chunk, eight 16-byte pieces per pixel straight from the NHWC
 // activations with cp.async (zero-fill outside the image / beyond R), into the 128B-swizzled K-major layout the
 // sparse kernel uses. Thin layers (Cin = 16, 32) pack 4 or 2 filter taps into one 64-wide chunk, so a 3x3x16 filter
-// is 3 chunks instead of 9. Same warp roles as spconv_tc.cu: warps 0-3 gather then run the epilogue (TMEM lane =
-// pixel), warp 4 allocates TMEM and issues tcgen05.mma; full/empty mbarrier ring, tcgen05.commit frees stages.
+// is 3 chunks instead of 9. Same thread roles as spconv_tc.cu: threads 0-255 = two consumer warpgroups issuing wgmma
+// (64 pixels each, accumulator in registers, written to shared memory at the end of the tile), threads 256-383 gather
+// then run the epilogue (thread = pixel); full/empty mbarrier ring.
 //
 // The input gradient is the same kernel in transposed-gather mode; the weight gradient is a second kernel below with
 // the pixels as the reduction dimension (split-K).
@@ -26,7 +27,7 @@ using namespace esb_tc;
 namespace {
 
 template <int N_TILE, int STAGES>
-__global__ void __launch_bounds__(160)
+__global__ void __launch_bounds__(384, 1)
 conv2d_tc_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ wt,
                      const float* __restrict__ bias, const __nv_bfloat16* __restrict__ res,
                      __nv_bfloat16* __restrict__ y, long long M, int H, int W, int cin, int Ho, int Wo, int cout, int kh,
@@ -34,14 +35,16 @@ conv2d_tc_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* _
   constexpr int B_STAGE_BYTES = N_TILE * 128;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   constexpr int LAG = STAGES - 2;
+  constexpr int NCONS = 256;
+  constexpr int PITCH = N_TILE + 4;                // floats per accumulator-image row
+  static_assert(TC_M * PITCH * 4 <= STAGES * STAGE_BYTES, "the accumulator image reuses the stage buffers");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = (uint64_t*)(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = (uint32_t*)(accum_bar + 1);
+  float* img = reinterpret_cast<float*>(smem);
 
-  const int warp = threadIdx.x >> 5;
   const long long tile = blockIdx.x;
   const int n0 = blockIdx.y * N_TILE;
   const int total = r_pad / TC_BK;                 // >= 1
@@ -49,20 +52,16 @@ conv2d_tc_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* _
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 128);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], NCONS / 32);
     }
-    mbar_init(accum_bar, 1);
+    mbar_init(accum_bar, NCONS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) tmem_alloc(tmem_slot, N_TILE);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp < 4) {
+  if (threadIdx.x >= NCONS) {
     // ---------------- producers: 8 lanes fetch the 8 x 16 B pieces of one pixel's chunk (see spconv_tc.cu) ----------
-    const int t = threadIdx.x;
+    const int t = threadIdx.x - NCONS;
     const int sub = t & 7, rgrp = t >> 3;
     const uint32_t sw = (uint32_t)(rgrp & 7);
     const uint32_t a_thread_off = (uint32_t)((rgrp >> 3) * 1024 + (rgrp & 7) * 128) + ((sub ^ sw) << 4);
@@ -133,13 +132,12 @@ conv2d_tc_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* _
     for (int d = (total > LAG ? total - LAG : 0); d < total; ++d) mbar_arrive(&full_bar[d % STAGES]);
 
     // ---------------- epilogue: + bias, + residual, ReLU, bf16 ----------------
-    const long long row = tile * TC_M + threadIdx.x;        // TMEM lane = pixel of the tile
+    const long long row = tile * TC_M + t;                  // accumulator-image row = pixel of the tile
     mbar_wait(accum_bar, 0);
-    tc_fence_after();
 #pragma unroll 1
     for (int c0 = 0; c0 < N_TILE; c0 += 32) {
       uint32_t v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
+      img_ld<32>(img, PITCH, t, c0, v);
       if (row < M) {
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
@@ -178,32 +176,28 @@ conv2d_tc_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* _
         }
       }
     }
-    tc_fence_before();
   } else {
-    // ---------------- MMA issuer (warp 4) ----------------
-    const uint32_t idesc = make_idesc(TC_M, N_TILE, 0, 0);
+    // ---------------- consumers: warpgroup wg owns pixels 64 wg .. 64 wg + 63 of the tile ----------------
+    const int wg = threadIdx.x >> 7;
+    float acc[N_TILE / 2];
     for (int it = 0; it < total; ++it) {
       const int s = it % STAGES;
       mbar_wait(&full_bar[s], (it / STAGES) & 1);
-      tc_fence_after();
-      if ((threadIdx.x & 31) == 0) {
-        const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
-        const uint32_t b_addr = a_addr + A_STAGE_BYTES;
+      const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES) + wg * 8192;
+      const uint32_t b_addr = smem_u32(smem + s * STAGE_BYTES) + A_STAGE_BYTES;
+      wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < TC_BK / 16; ++kk)
-          umma_bf16(tmem_base, make_desc(a_addr + kk * 32, 16, 1024), make_desc(b_addr + kk * 32, 16, 1024), idesc,
-                    (it > 0 || kk > 0) ? 1u : 0u);
-        umma_commit(&empty_bar[s]);
-        if (it == total - 1) umma_commit(accum_bar);
-      }
-      __syncwarp();
+      for (int kk = 0; kk < TC_BK / 16; ++kk)
+        wgmma_bf16<N_TILE, 0, 0>(acc, make_desc(a_addr + kk * 32, 16, 1024), make_desc(b_addr + kk * 32, 16, 1024), it > 0 || kk > 0);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (it > 0 && (threadIdx.x & 31) == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, N_TILE);
+    wgmma_wait<0>();
+    acc_fence<N_TILE / 2>(acc);
+    asm volatile("bar.sync 2, %0;" ::"n"(NCONS) : "memory");
+    acc_store<N_TILE>(acc, img, PITCH, wg * 64, threadIdx.x & 127);
+    mbar_arrive(accum_bar);
   }
 }
 
@@ -216,7 +210,7 @@ int launch_conv2d(const void* x, const void* wt, const float* bias, const void* 
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { esb_set_error("conv2d_tc_fwd: smem attr: %s", cudaGetErrorString(e)); return ESB_ECUDA; }
   dim3 grid(esb_div_up(M, TC_M), esb_div_up(cout, N_TILE));
-  kern<<<grid, 160, smem, stream>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)wt, bias, (const __nv_bfloat16*)res,
+  kern<<<grid, 384, smem, stream>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)wt, bias, (const __nv_bfloat16*)res,
                                     (__nv_bfloat16*)y, M, H, W, cin, Ho, Wo, cout, kh, kw, stride, pad, r_pad, relu, transposed);
   return ESB_OK;
 }
@@ -229,7 +223,7 @@ int launch_conv2d(const void* x, const void* wt, const float* bias, const void* 
 // CTA = (chunk of pixels: split-K) x (128-wide slice of r) x (N_TILE slice of Cout); fp32 atomics into dW^T.
 // ------------------------------------------------------------------------------------------------------------
 template <int N_TILE, int STAGES>
-__global__ void __launch_bounds__(160)
+__global__ void __launch_bounds__(384, 1)
 conv2d_tc_wgrad_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy, float* __restrict__ dw,
                        long long M, int H, int W, int cin, int Ho, int Wo, int cout, int kh, int kw, int stride, int pad,
                        int chunk_pixels) {
@@ -237,14 +231,15 @@ conv2d_tc_wgrad_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16*
   constexpr int B_BYTES = 64 * N_TILE * 2;
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   constexpr int LAG = STAGES - 2;
+  constexpr int NCONS = 256;
+  constexpr int PITCH = N_TILE + 4;
+  static_assert(128 * PITCH * 4 <= STAGES * STAGE_BYTES, "the accumulator image reuses the stage buffers");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = (uint64_t*)(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = (uint32_t*)(accum_bar + 1);
 
-  const int warp = threadIdx.x >> 5;
   const long long s_beg = (long long)blockIdx.x * chunk_pixels;
   const long long s_end = s_beg + chunk_pixels < M ? s_beg + chunk_pixels : M;
   if (s_beg >= M) return;                          // uniform for the whole CTA
@@ -255,19 +250,16 @@ conv2d_tc_wgrad_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16*
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 128);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], NCONS / 32);
     }
-    mbar_init(accum_bar, 1);
+    mbar_init(accum_bar, NCONS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) tmem_alloc(tmem_slot, N_TILE);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp < 4) {
-    const int t = threadIdx.x;
+  if (threadIdx.x >= NCONS) {
+    const int t = threadIdx.x - NCONS;
+    const int warp = t >> 5;
     // thread t moves 16-byte piece (t & 15) of pixel rows kk = (t >> 4) + 8 q, q = 0..7; its 8 reduction elements
     // r = r0 + 8 (t & 15) .. +7 lie in ONE filter tap (cin % 8 == 0), fixed for the whole kernel
     const int mc = t & 15, kk0 = t >> 4;
@@ -320,59 +312,43 @@ conv2d_tc_wgrad_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16*
     fence_proxy_async();
     for (int d = (total > LAG ? total - LAG : 0); d < total; ++d) mbar_arrive(&full_bar[d % STAGES]);
 
-    // epilogue: TMEM lane = reduction element r (within the 128 slice), column = co; transposed through the idle stage
-    // buffers so a warp adds contiguous runs of one dW^T row with 16-byte vector atomics (see spconv_tc_wgrad_kernel)
+    // epilogue: image row = reduction element r (within the 128 slice), column = co; a warp stores contiguous runs of one
+    // row of this pixel chunk's partial of dW^T (the host adds the chunks in order)
     mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    constexpr int PITCH = N_TILE + 4;
-    float* stg = reinterpret_cast<float*>(smem);
-#pragma unroll 1
-    for (int c0 = 0; c0 < N_TILE; c0 += 32) {
-      uint32_t v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        *reinterpret_cast<float4*>(stg + threadIdx.x * PITCH + c0 + 4 * q) =
-            make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                        __uint_as_float(v[4 * q + 3]));
-    }
-    tc_fence_before();
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    const int lane = threadIdx.x & 31;
+    const float* stg = reinterpret_cast<const float*>(smem);
+    const int lane = t & 31;
     for (int i = 0; i < 32; ++i) {
       const int rl = warp * 32 + i;
       const int rr = r0 + rl;
       if (rr >= R) break;
-      float* dwrow = dw + (long long)rr * cout + co0;
+      float* dwrow = dw + ((long long)blockIdx.x * R + rr) * cout + co0;
 #pragma unroll
       for (int c = lane * 4; c < N_TILE; c += 128)
         if (co0 + c < cout)                              // cout % 8 == 0: a float4 is all in or all out
-          atomicAdd(reinterpret_cast<float4*>(dwrow + c), *reinterpret_cast<const float4*>(stg + rl * PITCH + c));
+          *reinterpret_cast<float4*>(dwrow + c) = *reinterpret_cast<const float4*>(stg + rl * PITCH + c);
     }
   } else {
-    const uint32_t idesc = make_idesc(128, N_TILE, 1, 1);
+    // consumers: warpgroup wg owns reduction rows r0 + 64 wg .. (the second MN atom of the A tile)
+    const int wg = threadIdx.x >> 7;
+    float acc[N_TILE / 2];
     for (int it = 0; it < total; ++it) {
       const int s = it % STAGES;
       mbar_wait(&full_bar[s], (it / STAGES) & 1);
-      tc_fence_after();
-      if ((threadIdx.x & 31) == 0) {
-        const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
-        const uint32_t b_addr = a_addr + A_BYTES;
+      const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES) + wg * 8192;
+      const uint32_t b_addr = smem_u32(smem + s * STAGE_BYTES) + A_BYTES;
+      wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)              // 16 pixels per MMA = two 8-row K groups = 2048 B
-          umma_bf16(tmem_base, make_desc(a_addr + kk * 2048, 8192, 1024), make_desc(b_addr + kk * 2048, 8192, 1024),
-                    idesc, (it > 0 || kk > 0) ? 1u : 0u);
-        umma_commit(&empty_bar[s]);
-        if (it == total - 1) umma_commit(accum_bar);
-      }
-      __syncwarp();
+      for (int kk = 0; kk < 4; ++kk)              // 16 pixels per MMA = two 8-row K groups = 2048 B
+        wgmma_bf16<N_TILE, 1, 1>(acc, make_desc(a_addr + kk * 2048, 8192, 1024), make_desc(b_addr + kk * 2048, 8192, 1024), it > 0 || kk > 0);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (it > 0 && (threadIdx.x & 31) == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, N_TILE);
+    wgmma_wait<0>();
+    acc_fence<N_TILE / 2>(acc);
+    asm volatile("bar.sync 2, %0;" ::"n"(NCONS) : "memory");
+    acc_store<N_TILE>(acc, reinterpret_cast<float*>(smem), PITCH, wg * 64, threadIdx.x & 127);
+    mbar_arrive(accum_bar);
   }
 }
 
@@ -384,9 +360,14 @@ int launch_conv2d_wgrad(const void* x, const void* dy, float* dw, long long M, i
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { esb_set_error("conv2d_tc_wgrad: smem attr: %s", cudaGetErrorString(e)); return ESB_ECUDA; }
   dim3 grid(esb_div_up(M, chunk_pixels), esb_div_up(kh * kw * cin, 128), esb_div_up(cout, N_TILE));
-  kern<<<grid, 160, smem, stream>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)dy, dw, M, H, W, cin, Ho, Wo, cout, kh,
+  const long long width = (long long)kh * kw * cin * cout;     // every pixel chunk writes a whole partial of dW^T
+  float* part = nullptr;
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, sizeof(float) * grid.x * width, stream));
+  kern<<<grid, 384, smem, stream>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)dy, part, M, H, W, cin, Ho, Wo, cout, kh,
                                     kw, stride, pad, chunk_pixels);
-  return ESB_OK;
+  int rc = esb_sum_partial_rows(part, (int)grid.x, width, dw, 1, stream);
+  ESB_CUDA_CALL(esb_scratch_free(part, stream));
+  return rc;
 }
 
 }  // namespace
@@ -398,10 +379,10 @@ static int conv2d_dispatch(const void* x, const void* w, const float* bias, cons
   int rc;
 #define ESB_C2D(NT, ST) \
   launch_conv2d<NT, ST>(x, w, bias, residual, y, M, Hs, Ws, cs, Hr, Wr, cr, kh, kw, stride, pad, r_pad, relu, transposed, stream)
-  if (cr > 128 && row_tiles * ((cr + 255) / 256) >= 148)
+  if (cr > 128 && row_tiles * ((cr + 255) / 256) >= esb_sm_count())
     rc = ESB_C2D(256, 4);
   else if (cr > 64)
-    rc = ESB_C2D(128, 3);
+    rc = ESB_C2D(128, 4);
   else if (cr > 32)
     rc = ESB_C2D(64, 4);
   else
@@ -443,7 +424,7 @@ extern "C" int esb_conv2d_tc_dgrad(const void* dy, const void* w_ihwo, void* dx,
                          (cudaStream_t)stream_);
 }
 
-// Weight gradient: dw_t (kh*kw*cin, cout) fp32, ZEROED BY THE CALLER (split-K partial sums arrive through fp32 atomics),
+// Weight gradient: dw_t (kh*kw*cin, cout) fp32 += the gradient (zeroed by the caller; split-K partials are added in order),
 // row r = (ky, kx, ci) like the forward's reduction index: dW[co, ci, ky, kx] = dw_t[(ky*kw + kx)*cin + ci, co].
 extern "C" int esb_conv2d_tc_wgrad(const void* x, const void* dy, float* dw_t, int n_img, int H, int W, int cin, int cout,
                                    int kh, int kw, int stride, int pad, void* stream_) {
@@ -456,7 +437,7 @@ extern "C" int esb_conv2d_tc_wgrad(const void* x, const void* dy, float* dw_t, i
   const int n_tile = cout > 64 ? 128 : 64;
   // ~4 waves of 2 CTAs per SM over the (r-slice, channel-tile) grid; chunks of whole 64-pixel stages
   const long long tiles = (long long)esb_div_up(kh * kw * cin, 128) * esb_div_up(cout, n_tile);
-  const long long target_chunks = (4LL * 296 + tiles - 1) / tiles;
+  const long long target_chunks = (4LL * 2 * esb_sm_count() + tiles - 1) / tiles;
   long long cp = (M + target_chunks - 1) / target_chunks;
   cp = (cp + 63) / 64 * 64;
   if (cp < 512) cp = 512;

@@ -1,4 +1,4 @@
-// esb200 — dense NHWC convolution as a persistent TMA + tcgen05 implicit GEMM (bf16 in, fp32 accumulate in TMEM).
+// esb200 — dense NHWC convolution as a persistent TMA + wgmma implicit GEMM (bf16 in, fp32 accumulate).
 // The per-view image backbone of the hot path (SURVEY §8 row a5: mmdet.ResNet(depth=50, base_channels=16), called at
 // embodiedscan/models/detectors/sparse_featfusion_single_stage.py:130-136; config
 // configs/detection/mv-det3d_8xb4_embodiedscan-3d-284class-9dof.py:24-34) with the frozen BatchNorm folded into the
@@ -9,14 +9,15 @@
 //   * A CTA is persistent: it walks output tiles  (TN images x TH rows x TW columns <= 128 pixels) x (N_TILE channels).
 //   * A operand: for every filter tap ONE tiled TMA load of the box {bc channels, TW, TH, TN} of the NHWC activation tensor
 //     at the tap's spatial offset. Zero padding = TMA out-of-bounds fill; stride-2 convolutions use the tensor map's element
-//     strides. The box lands in shared memory as the K-major [pixel][channel] tile tcgen05 wants; thin layers (16 / 32
+//     strides. The box lands in shared memory as the K-major [pixel][channel] tile wgmma reads; thin layers (16 / 32
 //     channels) use the 32B / 64B swizzle modes and several taps share one pipeline stage.
 //   * B operand: 2-D TMA box of the OHWI filter matrix (row = output channel, columns = (tap, input channel)).
-//   * One elected thread issues tcgen05.mma (M=128, N=N_TILE, K=16) into one of two TMEM accumulator stages, so the epilogue
-//     of tile i overlaps the loads and MMAs of tile i+1.
-//   * Epilogue warps: tcgen05.ld -> + bias (+ residual) (ReLU) -> bf16 -> swizzled shared tile -> TMA store (the store
+//   * Two consumer warpgroups issue wgmma (m64, N=N_TILE, K=16), 64 tile rows each, accumulating in registers; at the end of
+//     a tile they write the accumulator to a shared-memory image, so the epilogue of tile i overlaps the loads and MMAs of
+//     tile i+1 (the registers are the second accumulator buffer).
+//   * Epilogue warps: image row -> + bias (+ residual) (ReLU) -> bf16 -> swizzled shared tile -> TMA store (the store
 //     clips partial tiles; no per-thread global stores).
-// Warp roles: 0 = TMA producer, 1 = TMEM allocator + MMA issuer, 2..5 = epilogue (TMEM lane quadrant = warp & 3).
+// Thread roles: 0..255 = consumer warpgroups, 256..287 = TMA producer warp, 288..415 = epilogue (thread = tile row).
 //
 // Roofline: HBM. Algorithmic bytes = (N*H*W*Cin + N*Ho*Wo*Cout [+ residual]) * 2 + kh*kw*Cin*Cout*2 per launch.
 #include "tc_common.cuh"
@@ -40,12 +41,14 @@ struct ConvGeom {
 };
 
 constexpr int EPI_THREADS = 128;
-constexpr int THREADS = 64 + EPI_THREADS;
+constexpr int NCONS = 256;                          // two consumer warpgroups
+constexpr int PROD0 = NCONS, EPI0 = NCONS + 32;     // first thread of the producer warp / of the epilogue warps
+constexpr int THREADS = EPI0 + EPI_THREADS;
 
 __device__ __forceinline__ uint32_t swz(uint32_t off, uint32_t mask) { return off ^ (((off >> 7) & mask) << 4); }
 
 template <int N_TILE, bool B_MN>
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(THREADS, 1)
 conv_tma_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmw,
                 const __grid_constant__ CUtensorMap tmy, const float* __restrict__ bias,
                 const __nv_bfloat16* __restrict__ res, const ConvGeom g) {
@@ -55,19 +58,19 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__
   constexpr uint32_t CB_MASK = CB_ROW_BYTES == 128 ? 7u : CB_ROW_BYTES == 64 ? 3u : 1u;
   constexpr int B_STAGE_BYTES = N_TILE * 128;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  constexpr int TMEM_COLS = 2 * N_TILE < 32 ? 32 : 2 * N_TILE;
+  constexpr int PITCH = N_TILE + 4;                            // floats per accumulator-image row
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   const int STAGES = g.stages;
   uint8_t* cbuf = smem + STAGES * STAGE_BYTES;                 // 2 x CB_BYTES, 1024-aligned (STAGE_BYTES % 1024 == 0)
-  uint64_t* full_bar = (uint64_t*)(cbuf + 2 * CB_BYTES);
+  float* img = reinterpret_cast<float*>(cbuf + 2 * CB_BYTES);  // 128 x PITCH accumulator image
+  uint64_t* full_bar = (uint64_t*)(img + 128 * PITCH);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tempty_bar + 2);
+  uint64_t* tfull_bar = empty_bar + STAGES;                    // image written (consumers -> epilogue)
+  uint64_t* tempty_bar = tfull_bar + 1;                        // image drained (epilogue -> consumers)
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int n_sub = g.ntaps * g.nchunk;                        // sub-tiles (tap, channel chunk) per output tile
   const int n_it = (n_sub + g.group - 1) / g.group;            // pipeline stages per output tile
   const int bcb = g.bc * 2;                                    // bytes per sub-tile row
@@ -79,24 +82,18 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], NCONS / 32);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], EPI_THREADS);
-    }
+    mbar_init(tfull_bar, NCONS);
+    mbar_init(tempty_bar, EPI_THREADS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmx);
     tma_prefetch_desc(&tmw);
     tma_prefetch_desc(&tmy);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (threadIdx.x >= PROD0 && threadIdx.x < EPI0) {
     // ------------------------------------------------ TMA producer ------------------------------------------------
     if (lane == 0) {
       uint32_t it = 0;
@@ -134,50 +131,51 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------ MMA issuer ------------------------------------------------
-    const uint32_t idesc = make_idesc(TC_M, N_TILE, 0, B_MN ? 1 : 0);
-    const uint32_t a_layout = umma_layout_of(bcb);
+  } else if (threadIdx.x < NCONS) {
+    // ------------------------------------------------ consumers ------------------------------------------------
+    const int wg = threadIdx.x >> 7;                           // tile rows 64 wg .. 64 wg + 63
+    const uint32_t a_layout = mma_layout_of(bcb);
     uint32_t it = 0, tcount = 0;
+    float acc[N_TILE / 2];
     for (int work = blockIdx.x; work < n_work; work += gridDim.x, ++tcount) {
-      const uint32_t as = tcount & 1;
-      mbar_wait(&tempty_bar[as], ((tcount >> 1) & 1) ^ 1);     // epilogue has drained this accumulator stage
-      tc_fence_after();
-      const uint32_t tacc = tmem_base + as * N_TILE;
+      int prev = -1;
       for (int i = 0; i < n_it; ++i, ++it) {
         const int s = it % STAGES;
         mbar_wait(&full_bar[s], (it / STAGES) & 1);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t a_base = smem_u32(smem + s * STAGE_BYTES);
-          const uint32_t b_base = a_base + A_STAGE_BYTES;
-          const int cnt = min(g.group, n_sub - i * g.group);
-          for (int j = 0; j < cnt; ++j) {
-            const uint32_t a_sub = a_base + j * (128 * bcb), b_sub = b_base + j * b_sub_bytes;
-            for (int kk = 0; kk < g.bc / 16; ++kk) {
-              const uint64_t ad = make_desc_sw(a_sub + kk * 32, 16, 8 * bcb, a_layout);
-              uint64_t bd;
-              if (!B_MN) {
-                bd = make_desc_sw(b_sub + kk * 32, 16, 8 * bcb, a_layout);
-              } else {
-                constexpr int NAB = (N_TILE < 64 ? N_TILE : 64) * 2;     // bytes per MN-major row (one atom of columns)
-                bd = make_desc_sw(b_sub + kk * 16 * NAB, g.bc * NAB, 8 * NAB, umma_layout_of(NAB));
-              }
-              umma_bf16(tacc, ad, bd, idesc, (i > 0 || j > 0 || kk > 0) ? 1u : 0u);
+        const uint32_t a_base = smem_u32(smem + s * STAGE_BYTES);
+        const uint32_t b_base = a_base + A_STAGE_BYTES;
+        const int cnt = min(g.group, n_sub - i * g.group);
+        wgmma_fence();
+        for (int j = 0; j < cnt; ++j) {
+          const uint32_t a_sub = a_base + j * (128 * bcb) + wg * (64 * bcb), b_sub = b_base + j * b_sub_bytes;
+          for (int kk = 0; kk < g.bc / 16; ++kk) {
+            const uint64_t ad = make_desc_sw(a_sub + kk * 32, 16, 8 * bcb, a_layout);
+            const int accumulate = i > 0 || j > 0 || kk > 0;
+            if (!B_MN) {
+              wgmma_bf16<N_TILE, 0, 0>(acc, ad, make_desc_sw(b_sub + kk * 32, 16, 8 * bcb, a_layout), accumulate);
+            } else {
+              constexpr int NAB = (N_TILE < 64 ? N_TILE : 64) * 2;     // bytes per MN-major row (one atom of columns)
+              wgmma_bf16<N_TILE, 0, 1>(acc, ad, make_desc_sw(b_sub + kk * 16 * NAB, g.bc * NAB, 8 * NAB, mma_layout_of(NAB)),
+                                       accumulate);
             }
           }
-          umma_commit(&empty_bar[s]);                          // stage reusable once these MMAs have read it
-          if (i == n_it - 1) umma_commit(&tfull_bar[as]);      // accumulator complete
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();                                       // the group of the previous stage has retired
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = s;
       }
+      wgmma_wait<0>();
+      acc_fence<N_TILE / 2>(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      mbar_wait(tempty_bar, (tcount & 1) ^ 1);                 // the epilogue has drained the previous tile's image
+      acc_store<N_TILE>(acc, img, PITCH, wg * 64, threadIdx.x & 127);
+      mbar_arrive(tfull_bar);
     }
-    tc_fence_before();
   } else {
     // ------------------------------------------------ epilogue ------------------------------------------------
-    const int et = threadIdx.x - 64;                           // 0..127
-    const int quad = warp & 3;                                 // TMEM lane quadrant this warp may read
-    const int m = quad * 32 + lane;                            // tile row = TMEM lane
+    const int et = threadIdx.x - EPI0;                         // 0..127
+    const int m = et;                                          // tile row = image row
     uint32_t tcount = 0, cb = 0;
     for (int work = blockIdx.x; work < n_work; work += gridDim.x, ++tcount) {
       int t = work;
@@ -195,10 +193,7 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__
       const int mi = mr / g.TD;
       const bool valid = m < rows_box && img0 + mi < g.N && od0 + md < g.Do && oh0 + mh < g.Ho && ow0 + mw < g.Wo;
       const long long pix = (((long long)(img0 + mi) * g.Do + (od0 + md)) * g.Ho + (oh0 + mh)) * g.Wo + (ow0 + mw);
-      const uint32_t as = tcount & 1;
-      mbar_wait(&tfull_bar[as], (tcount >> 1) & 1);
-      tc_fence_after();
-      const uint32_t tacc = tmem_base + ((uint32_t)(quad * 32) << 16) + as * N_TILE;
+      mbar_wait(tfull_bar, tcount & 1);
 #pragma unroll 1
       for (int c0 = 0; c0 < N_TILE; c0 += CB_COLS, cb ^= 1) {
         if (et == 0) tma_store_wait_read<1>();                 // the store issued from this buffer two chunks ago has read it
@@ -206,17 +201,10 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__
         uint8_t* crow = cbuf + cb * CB_BYTES;
 #pragma unroll 1
         for (int c1 = 0; c1 < CB_COLS; c1 += 32) {
-          constexpr int W32 = CB_COLS < 32 ? CB_COLS : 32;     // columns handled per TMEM load (16 or 32)
+          constexpr int W32 = CB_COLS < 32 ? CB_COLS : 32;     // columns handled per image read (16 or 32)
           uint32_t v[32];
-          if (W32 == 32) {
-            tmem_ld32(tacc + (uint32_t)(c0 + c1), v);
-          } else {
-            tmem_ld16(tacc + (uint32_t)(c0 + c1), v);
-          }
-          if (c0 + CB_COLS >= N_TILE && c1 + 32 >= CB_COLS) {  // last read of this accumulator stage
-            tc_fence_before();
-            mbar_arrive(&tempty_bar[as]);
-          }
+          img_ld<W32>(img, PITCH, m, c0 + c1, v);
+          if (c0 + CB_COLS >= N_TILE && c1 + 32 >= CB_COLS) mbar_arrive(tempty_bar);   // last read of this tile's image
 #pragma unroll
           for (int q = 0; q < W32 / 8; ++q) {
             const int c = n0 + c0 + c1 + 8 * q;
@@ -262,11 +250,6 @@ conv_tma_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__
     }
     if (et == 0) tma_store_wait<0>();                          // global writes complete before the kernel ends
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 // pick the output-tile extent (TW x TH x TD x TN <= 128 pixels) that wastes the fewest MMA rows over the whole output
@@ -289,24 +272,19 @@ int launch(const CUtensorMap& tmx, const CUtensorMap& tmw, const CUtensorMap& tm
            ConvGeom g, cudaStream_t stream) {
   constexpr int CB_COLS = N_TILE < 64 ? N_TILE : 64;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + N_TILE * 128;
-  const int n_it = (g.ntaps * g.nchunk + g.group - 1) / g.group;
-  (void)n_it;
+  constexpr int IMG_BYTES = 128 * (N_TILE + 4) * 4;
   // the stage ring runs ahead ACROSS output tiles (persistent CTA), so its depth is set by shared memory, not by the filter:
-  // two CTAs per SM up to N_TILE = 64 (~100 KB each), one CTA per SM above
-  const int budget = (N_TILE <= 64 ? 100 : 200) * 1024 - 2 * 128 * CB_COLS * 2;
+  // one CTA per SM, whatever the 227 KB per block leave after the accumulator image and the two store buffers
+  const int budget = 227 * 1024 - IMG_BYTES - 2 * 128 * CB_COLS * 2 - 2048;
   int stages = budget / STAGE_BYTES;
   stages = stages > 6 ? 6 : stages < 2 ? 2 : stages;
   g.stages = stages;
-  const size_t smem = (size_t)stages * STAGE_BYTES + 2 * 128 * CB_COLS * 2 + (2 * stages + 4) * 8 + 16 + 1024;
+  const size_t smem = (size_t)stages * STAGE_BYTES + 2 * 128 * CB_COLS * 2 + IMG_BYTES + (2 * stages + 2) * 8 + 1024;
   auto kern = conv_tma_kernel<N_TILE, B_MN>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { esb_set_error("conv_tma: smem attr (%zu B): %s", smem, cudaGetErrorString(e)); return ESB_ECUDA; }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long n_work = (long long)g.tiles_w * g.tiles_h * g.tiles_d * g.tiles_n * g.n_blocks;
-  const int per_sm = (smem <= 110 * 1024 && 2 * N_TILE * 2 <= 512) ? 2 : 1;
-  long long grid = (long long)sms * per_sm;
+  long long grid = esb_sm_count();
   if (grid > n_work) grid = n_work;
   kern<<<(unsigned)grid, THREADS, smem, stream>>>(tmx, tmw, tmy, bias, (const __nv_bfloat16*)res, g);
   return ESB_OK;
@@ -328,7 +306,7 @@ int conv_tma_run(const void* in, const void* w, const float* bias, const void* r
   choose_tile(Wo, Ho, Do, N, &g.TW, &g.TH, &g.TD, &g.TN);
   g.tiles_w = esb_div_up(Wo, g.TW); g.tiles_h = esb_div_up(Ho, g.TH); g.tiles_d = esb_div_up(Do, g.TD);
   g.tiles_n = esb_div_up(N, g.TN);
-  const int n_tile = Co >= 256 ? 256 : Co;
+  const int n_tile = Co >= 128 ? 128 : Co;                     // 64 accumulator registers per consumer thread at most
   g.n_blocks = Co / n_tile;
   const int sd = Di > 1 ? stride : 1;          // a depth-1 (2-D) problem has nothing to stride over
   CUtensorMap tmx, tmw, tmy;
@@ -374,8 +352,7 @@ int conv_tma_run(const void* in, const void* w, const float* bias, const void* r
     case 32: rc = ESB_CT(32); break;
     case 64: rc = ESB_CT(64); break;
     case 128: rc = ESB_CT(128); break;
-    case 256: rc = ESB_CT(256); break;
-    default: esb_set_error("conv_tma: unsupported output channel count %d (16, 32, 64, 128 or a multiple of 256)", Co); return ESB_EINVAL;
+    default: esb_set_error("conv_tma: unsupported output channel count %d (16, 32, 64 or a multiple of 128)", Co); return ESB_EINVAL;
   }
 #undef ESB_CT
   if (rc != ESB_OK) return rc;
@@ -507,9 +484,10 @@ extern "C" int esb_conv3d_tma_dgrad(const void* dy, const void* w_odhwi, void* d
 // ------------------------------------------------------------------------------------------------------------
 // The 7x7 / stride 2 / pad 3 stem on the 3-channel image (Cin = 3 cannot feed a 16-byte TMA box): the CTA stages the
 // input patch of a 16 x 8 output tile in shared memory with coalesced loads, every thread lays out ITS pixel's 147-tap row
-// as the K-major 128B-swizzled A operand (im2col in shared memory, never in HBM), one thread issues ten tcgen05.mma
-// (M=128, N=16, K=16) against the filter resident in shared memory, and the epilogue adds the folded-BN bias, applies
-// ReLU and stores 32 contiguous bytes per pixel. Persistent over tiles. Roofline: HBM (image in, 16-channel map out).
+// as the K-major 128B-swizzled A operand (im2col in shared memory, never in HBM), the warpgroup issues ten wgmma
+// (m64, N=16, K=16) per 64-row half against the filter resident in shared memory, writes the accumulator over the idle A tile,
+// and every thread adds the folded-BN bias to ITS pixel, applies ReLU and stores 32 contiguous bytes.
+// Persistent over tiles. Roofline: HBM (image in, 16-channel map out).
 // ------------------------------------------------------------------------------------------------------------
 namespace {
 
@@ -525,15 +503,10 @@ stem7x7_tc_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __re
   uint8_t* a_tile = smem;                                   // 3 chunks x (128 rows x 128 B) = 48 KB
   uint8_t* b_tile = smem + 3 * 16384;                       // 3 chunks x (16 rows x 128 B) = 6 KB
   __nv_bfloat16* patch = (__nv_bfloat16*)(b_tile + 3 * 2048);   // 21 x 112 bf16
-  uint64_t* bar = (uint64_t*)((uint8_t*)patch + ((ST_PH * ST_PW * 2 + 15) & ~15));
-  uint32_t* tmem_slot = (uint32_t*)(bar + 1);
+  float* acc_img = reinterpret_cast<float*>(a_tile);          // 128 x 20 fp32 accumulator image over the idle A tile
+  constexpr int PITCH = 20;
 
-  const int t = threadIdx.x, warp = t >> 5;
-  if (t == 0) {
-    mbar_init(bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) tmem_alloc(tmem_slot, 32);
+  const int t = threadIdx.x;
   // filter: (16, 147) bf16 -> K-major SW128 rows of three 64-wide chunks, zero beyond 147
   for (int i = t; i < 16 * 24; i += 128) {                  // 16 rows x 24 pieces of 8 elements
     const int n = i / 24, j = i - n * 24;                   // j = 16-byte piece index along K (0..23; 20..23 are padding)
@@ -546,16 +519,11 @@ stem7x7_tc_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __re
     const int c = j >> 3, jj = j & 7;
     *reinterpret_cast<uint4*>(b_tile + c * 2048 + n * 128 + ((jj ^ (n & 7)) << 4)) = make_uint4(v[0], v[1], v[2], v[3]);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t idesc = make_idesc(TC_M, 16, 0, 0);
 
   const int tiles_w = (Wo + ST_TW - 1) / ST_TW, tiles_h = (Ho + ST_TH - 1) / ST_TH;
   const int n_tiles = tiles_w * tiles_h * n_img;
   const int tx = t & 15, ty = t >> 4;                       // this thread's pixel inside the tile (row m = t)
-  uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     int r = tile;
     const int twi = r % tiles_w; r /= tiles_w;
@@ -592,23 +560,28 @@ stem7x7_tc_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __re
       }
     }
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    if (t == 0) {
+    {
       const uint32_t a_addr = smem_u32(a_tile), b_addr = smem_u32(b_tile);
+      float acc[2][8];
+      wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < ST_KPAD / 16; ++kk)
-        umma_bf16(tmem_base, make_desc(a_addr + (kk >> 2) * 16384 + (kk & 3) * 32, 16, 1024),
-                  make_desc(b_addr + (kk >> 2) * 2048 + (kk & 3) * 32, 16, 1024), idesc, kk > 0 ? 1u : 0u);
-      umma_commit(bar);
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int kk = 0; kk < ST_KPAD / 16; ++kk)
+          wgmma_bf16<16, 0, 0>(acc[h], make_desc(a_addr + h * 8192 + (kk >> 2) * 16384 + (kk & 3) * 32, 16, 1024),
+                               make_desc(b_addr + (kk >> 2) * 2048 + (kk & 3) * 32, 16, 1024), kk > 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence<8>(acc[0]);
+      acc_fence<8>(acc[1]);
+      __syncthreads();                                      // every MMA has read the A tile: the image may overwrite it
+      acc_store<16>(acc[0], acc_img, PITCH, 0, t);
+      acc_store<16>(acc[1], acc_img, PITCH, 64, t);
+      __syncthreads();
     }
-    mbar_wait(bar, phase);
-    phase ^= 1;
-    tc_fence_after();
     uint32_t v[32];
-    tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16), v);
-    tc_fence_before();
+    img_ld<16>(acc_img, PITCH, t, 0, v);
     const int ox = ox0 + tx, oy = oy0 + ty;
     if (ox < Wo && oy < Ho) {
       uint32_t o[8];
@@ -622,12 +595,7 @@ stem7x7_tc_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __re
       dst[0] = make_uint4(o[0], o[1], o[2], o[3]);
       dst[1] = make_uint4(o[4], o[5], o[6], o[7]);
     }
-    __syncthreads();          // the patch and the A tile are rewritten by the next iteration; TMEM reads are done
-  }
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 32);
+    __syncthreads();          // the patch and the A tile are rewritten by the next iteration; image reads are done
   }
 }
 
@@ -640,14 +608,11 @@ extern "C" int esb_stem7x7_tc(const void* x, const void* w_ohwi, const float* bi
   ESB_CHECK_ARG(bias != nullptr, "esb_stem7x7_tc: bias (16 fp32) is required");
   if (n_img == 0) return ESB_OK;
   const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
-  const size_t smem = 3 * 16384 + 3 * 2048 + ((ST_PH * ST_PW * 2 + 15) & ~15) + 16 + 1024;
+  const size_t smem = 3 * 16384 + 3 * 2048 + ((ST_PH * ST_PW * 2 + 15) & ~15) + 1024;
   cudaError_t e = cudaFuncSetAttribute(stem7x7_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { esb_set_error("esb_stem7x7_tc: smem attr: %s", cudaGetErrorString(e)); return ESB_ECUDA; }
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long n_tiles = (long long)esb_div_up(Wo, ST_TW) * esb_div_up(Ho, ST_TH) * n_img;
-  long long grid = (long long)sms * 3;
+  long long grid = (long long)esb_sm_count() * 3;
   if (grid > n_tiles) grid = n_tiles;
   stem7x7_tc_kernel<<<(unsigned)grid, 128, smem, (cudaStream_t)stream_>>>(
       (const __nv_bfloat16*)x, (const __nv_bfloat16*)w_ohwi, bias, (__nv_bfloat16*)y, n_img, H, W, Ho, Wo, relu);
@@ -660,10 +625,11 @@ extern "C" int esb_stem7x7_tc(const void* x, const void* w_ohwi, const float* bi
 // x[pixel shifted by tap, ci] * dy[pixel, co]. The pixels are the reduction dimension: a pipeline stage holds a box of exactly
 // 64 output pixels (TN x TH x TW, powers of two) of dy and, for every (tap, channel slice) "atom" of the CTA's 128-row slice
 // of the filter, the same box of x at the tap's offset (zero padding and ragged edges = TMA out-of-bounds zeros on BOTH
-// operands, stride 2 = element strides). Both boxes land as [pixel][channel] rows = the MN-major operands tcgen05 takes
-// directly (no transpose anywhere). A CTA accumulates its share of the pixel tiles in TMEM and adds its 128 x N_TILE fp32
-// tile to dW^T with coalesced 16-byte vector atomics.
-// CTA = (pixel-tile range) x (128-row slice of (tap, ci)) x (N_TILE slice of co). Warps: 0 producer, 1 MMA, 2..5 epilogue.
+// operands, stride 2 = element strides). Both boxes land as [pixel][channel] rows = the MN-major operands wgmma takes
+// directly (no transpose anywhere). A CTA accumulates its share of the pixel tiles in registers and stores its 128 x N_TILE
+// fp32 tile to its split's partial of dW^T; the host adds the splits in order.
+// CTA = (pixel-tile range) x (128-row slice of (tap, ci)) x (N_TILE slice of co). Threads: 0..255 consumers (64 filter rows
+// per warpgroup), 256..287 producer, 288..415 epilogue.
 // ------------------------------------------------------------------------------------------------------------
 namespace {
 
@@ -676,23 +642,23 @@ struct WgradGeom {
 };
 
 template <int N_TILE>
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(THREADS, 1)
 conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmdy,
                       float* __restrict__ dw, const WgradGeom g) {
   constexpr int NA = N_TILE < 64 ? N_TILE : 64;                // columns per B atom
   constexpr int A_BYTES = 64 * 256;                            // 64 pixels x 128 filter rows
   constexpr int B_BYTES = 64 * N_TILE * 2;
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  constexpr int TMEM_COLS = N_TILE < 32 ? 32 : N_TILE;
+  constexpr int PITCH = N_TILE + 4;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   const int STAGES = g.stages;
   uint64_t* full_bar = (uint64_t*)(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = (uint32_t*)(accum_bar + 1);
+  float* img = reinterpret_cast<float*>(smem);                 // accumulator image over the idle stage buffers
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int taps = g.kd * g.kh * g.kw;
   const int n_tiles = g.tiles_w * g.tiles_h * g.tiles_d * g.tiles_n;
   const int t_beg = blockIdx.x * g.tiles_per_cta;
@@ -709,20 +675,16 @@ conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_cons
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], NCONS / 32);
     }
-    mbar_init(accum_bar, 1);
+    mbar_init(accum_bar, NCONS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmx);
     tma_prefetch_desc(&tmdy);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (threadIdx.x >= PROD0 && threadIdx.x < EPI0) {
     if (lane == 0) {
       for (int it = 0; it < total; ++it) {
         int t = t_beg + it;
@@ -748,48 +710,35 @@ conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_cons
           tma_load_5d(&tmdy, &full_bar[s], b_base + b * (64 * NA * 2), co0 + b * NA, ox0, oy0, oz0, img0);
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = make_idesc(128, N_TILE, 1, 1);
-    const uint32_t a_layout = umma_layout_of(awb), b_layout = umma_layout_of(NA * 2);
+  } else if (threadIdx.x < NCONS) {
+    // consumers: warpgroup wg owns filter rows 64 wg .. 64 wg + 63 of the slice (64 / aw atoms further along the A tile)
+    const int wg = threadIdx.x >> 7;
+    const uint32_t a_layout = mma_layout_of(awb), b_layout = mma_layout_of(NA * 2);
+    float acc[N_TILE / 2];
     for (int it = 0; it < total; ++it) {
       const int s = it % STAGES;
       mbar_wait(&full_bar[s], (it / STAGES) & 1);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
-        const uint32_t b_addr = a_addr + A_BYTES;
+      const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES) + wg * (64 / g.aw) * a_atom_bytes;
+      const uint32_t b_addr = smem_u32(smem + s * STAGE_BYTES) + A_BYTES;
+      wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)                           // 16 pixels per MMA
-          umma_bf16(tmem_base, make_desc_sw(a_addr + kk * 16 * awb, a_atom_bytes, 8 * awb, a_layout),
-                    make_desc_sw(b_addr + kk * 16 * (NA * 2), 64 * NA * 2, 8 * (NA * 2), b_layout), idesc,
-                    (it > 0 || kk > 0) ? 1u : 0u);
-        umma_commit(&empty_bar[s]);
-        if (it == total - 1) umma_commit(accum_bar);
-      }
-      __syncwarp();
+      for (int kk = 0; kk < 4; ++kk)                           // 16 pixels per MMA
+        wgmma_bf16<N_TILE, 1, 1>(acc, make_desc_sw(a_addr + kk * 16 * awb, a_atom_bytes, 8 * awb, a_layout),
+                                 make_desc_sw(b_addr + kk * 16 * (NA * 2), 64 * NA * 2, 8 * (NA * 2), b_layout), it > 0 || kk > 0);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (it > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
     }
-    tc_fence_before();
+    wgmma_wait<0>();
+    acc_fence<N_TILE / 2>(acc);
+    asm volatile("bar.sync 2, %0;" ::"n"(NCONS) : "memory");  // every wgmma has read its stage: the image may overwrite them
+    acc_store<N_TILE>(acc, img, PITCH, wg * 64, threadIdx.x & 127);
+    mbar_arrive(accum_bar);
   } else {
-    const int quad = warp & 3;
-    const int et = quad * 32 + lane;
+    // epilogue: image row = filter row of the slice, column = co
+    const int quad = (threadIdx.x - EPI0) >> 5;
     mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    constexpr int PITCH = N_TILE + 4;
-    float* stg = reinterpret_cast<float*>(smem);
-#pragma unroll 1
-    for (int c0 = 0; c0 < N_TILE; c0 += 32) {
-      constexpr int W32 = N_TILE < 32 ? N_TILE : 32;
-      uint32_t v[32];
-      if (W32 == 32) tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)c0, v);
-      else tmem_ld16(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)c0, v);
-#pragma unroll
-      for (int q = 0; q < W32 / 4; ++q)
-        *reinterpret_cast<float4*>(stg + et * PITCH + c0 + 4 * q) =
-            make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                        __uint_as_float(v[4 * q + 3]));
-    }
-    tc_fence_before();
-    asm volatile("bar.sync 1, 128;" ::: "memory");
+    const float* stg = img;
     const int rows_valid = n_valid * g.aw;                       // accumulator rows backed by loaded atoms
     for (int rr = 0; rr < 32; ++rr) {
       const int r = quad * 32 + rr;
@@ -797,15 +746,10 @@ conv_tma_wgrad_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_cons
       // row r of the slice = atom r / aw, channel r % aw  ->  filter row (tap * cin + ch)
       const int ga = atom0 + r / g.aw;
       const int tap = ga / g.chunks_per_tap, ch = (ga - tap * g.chunks_per_tap) * g.aw + (r % g.aw);
-      float* dwrow = dw + ((long long)tap * g.cin + ch) * g.cout + co0;
+      float* dwrow = dw + (((long long)blockIdx.x * g.kd * g.kh * g.kw + tap) * g.cin + ch) * g.cout + co0;
       for (int c = lane * 4; c < N_TILE; c += 128)
-        atomicAdd(reinterpret_cast<float4*>(dwrow + c), *reinterpret_cast<const float4*>(stg + r * PITCH + c));
+        *reinterpret_cast<float4*>(dwrow + c) = *reinterpret_cast<const float4*>(stg + r * PITCH + c);
     }
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
@@ -823,13 +767,19 @@ int launch_wgrad_tma(const CUtensorMap& tmx, const CUtensorMap& tmdy, float* dw,
   if (e != cudaSuccess) { esb_set_error("conv_tma_wgrad: smem attr: %s", cudaGetErrorString(e)); return ESB_ECUDA; }
   const long long n_tiles = (long long)g.tiles_w * g.tiles_h * g.tiles_d * g.tiles_n;
   // ~2 CTAs per SM in total; every CTA walks a contiguous range of pixel tiles
-  long long splits = (2LL * 148 + (long long)slices * n_blocks - 1) / ((long long)slices * n_blocks);
+  long long splits = (2LL * esb_sm_count() + (long long)slices * n_blocks - 1) / ((long long)slices * n_blocks);
   if (splits > n_tiles) splits = n_tiles;
   if (splits < 1) splits = 1;
   g.tiles_per_cta = (int)((n_tiles + splits - 1) / splits);
   dim3 grid((unsigned)((n_tiles + g.tiles_per_cta - 1) / g.tiles_per_cta), slices, n_blocks);
-  kern<<<grid, THREADS, smem, stream>>>(tmx, tmdy, dw, g);
-  return ESB_OK;
+  // every split writes a whole partial of dW^T (its slices x channel blocks cover all rows and columns)
+  const long long width = (long long)g.kd * g.kh * g.kw * g.cin * g.cout;
+  float* part = nullptr;
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, sizeof(float) * grid.x * width, stream));
+  kern<<<grid, THREADS, smem, stream>>>(tmx, tmdy, part, g);
+  int rc = esb_sum_partial_rows(part, (int)grid.x, width, dw, 1, stream);
+  ESB_CUDA_CALL(esb_scratch_free(part, stream));
+  return rc;
 }
 
 }  // namespace
@@ -903,7 +853,7 @@ int conv_wgrad_any(const char* who, const void* x, const void* dy, float* dw_t, 
 
 }  // namespace
 
-// dw_t (kh*kw*cin, cout) fp32, ZEROED BY THE CALLER: dW[co, ci, ky, kx] = dw_t[(ky*kw + kx)*cin + ci, co].
+// dw_t (kh*kw*cin, cout) fp32 += the weight gradient (zeroed by the caller): dW[co, ci, ky, kx] = dw_t[(ky*kw + kx)*cin + ci, co].
 // x (n,H,W,cin), dy (n,Ho,Wo,cout) bf16 NHWC; cin, cout in {16, 32, 64, 128, 256, 512, ...}.
 extern "C" int esb_conv2d_tma_wgrad(const void* x, const void* dy, float* dw_t, int n_img, int H, int W, int cin, int cout,
                                     int kh, int kw, int stride, int pad, void* stream_) {
@@ -911,7 +861,7 @@ extern "C" int esb_conv2d_tma_wgrad(const void* x, const void* dy, float* dw_t, 
                         (cudaStream_t)stream_);
 }
 
-// 3-D: dw_t (k*k*k*cin, cout) fp32 zeroed by the caller, row = ((kz*k + ky)*k + kx)*cin + ci; x (n,D,H,W,cin), dy NDHWC bf16.
+// 3-D: dw_t (k*k*k*cin, cout) fp32 += the gradient (zeroed by the caller), row = ((kz*k + ky)*k + kx)*cin + ci; x (n,D,H,W,cin), dy NDHWC bf16.
 extern "C" int esb_conv3d_tma_wgrad(const void* x, const void* dy, float* dw_t, int n, int D, int H, int W, int cin, int cout, int k,
                                     int stride, int pad, void* stream_) {
   return conv_wgrad_any("esb_conv3d_tma_wgrad", x, dy, dw_t, n, D, H, W, cin, cout, k, k, k, stride, pad, (cudaStream_t)stream_);

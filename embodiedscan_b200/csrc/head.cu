@@ -255,7 +255,7 @@ __global__ void focal_fwd_kernel(const T* __restrict__ logits, const long long* 
   if (threadIdx.x == 0) {
     float s = 0.f;
     for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += red[i];
-    atomicAdd(loss_sum, s);
+    loss_sum[blockIdx.x] = s;                              // one partial per block, summed in block order
   }
 }
 
@@ -466,7 +466,10 @@ bbox_cd_loss_kernel(const float* __restrict__ points, const float* __restrict__ 
     for (int i = 0; i < 12; ++i) grad[p * 12 + i] = acc.d[i] * w;
   }
   lval = esb_warp_sum(lval);
-  if ((threadIdx.x & 31) == 0 && lval != 0.f) atomicAdd(loss_out, lval);
+  __shared__ float red[2];
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = lval;
+  __syncthreads();
+  if (threadIdx.x == 0) loss_out[blockIdx.x] = red[0] + red[1];   // one partial per 64-thread block, summed in block order
 }
 
 }  // namespace
@@ -518,14 +521,18 @@ extern "C" int esb_fcaf3d_targets(const float* points, const int* level_off, int
 extern "C" int esb_focal_loss_fwd(const void* logits, const long long* target, long long n, int C, float gamma,
                                   float alpha, const float* row_w, float* loss_sum, int dtype, void* stream) {
   if (n == 0) return ESB_OK;
+  cudaStream_t s = (cudaStream_t)stream;
   int grid = esb_div_up(n * C, 256);
+  float* part = nullptr;
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, (size_t)grid * sizeof(float), s));
   if (dtype == ESB_F32)
-    focal_fwd_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)logits, target, n, C, gamma, alpha, row_w, loss_sum);
+    focal_fwd_kernel<float><<<grid, 256, 0, s>>>((const float*)logits, target, n, C, gamma, alpha, row_w, part);
   else
-    focal_fwd_kernel<__nv_bfloat16><<<grid, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)logits, target, n, C, gamma,
-                                                                             alpha, row_w, loss_sum);
+    focal_fwd_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((const __nv_bfloat16*)logits, target, n, C, gamma, alpha, row_w, part);
   ESB_CUDA_LAUNCH_CHECK("focal_fwd_kernel");
-  return ESB_OK;
+  int rc = esb_sum_partial_rows(part, grid, 1, loss_sum, 1, s);
+  ESB_CUDA_CALL(esb_scratch_free(part, s));
+  return rc;
 }
 
 extern "C" int esb_focal_loss_bwd(const void* logits, const long long* target, long long n, int C, float gamma,
@@ -549,9 +556,14 @@ extern "C" int esb_focal_loss_bwd(const void* logits, const long long* target, l
 extern "C" int esb_bbox_cd_loss(const float* points, const float* bbox_pred, const float* targets, const float* row_w,
                                 const float* w4_host, int P, float* loss_out, float* grad, void* stream) {
   if (P == 0) return ESB_OK;
-  bbox_cd_loss_kernel<<<esb_div_up(P, 64), 64, 0, (cudaStream_t)stream>>>(points, bbox_pred, targets, row_w, w4_host[0],
-                                                                         w4_host[1], w4_host[2], w4_host[3], P, loss_out,
-                                                                         grad);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int grid = esb_div_up(P, 64);
+  float* part = nullptr;
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, (size_t)grid * sizeof(float), s));
+  bbox_cd_loss_kernel<<<grid, 64, 0, s>>>(points, bbox_pred, targets, row_w, w4_host[0], w4_host[1], w4_host[2], w4_host[3], P,
+                                          part, grad);
   ESB_CUDA_LAUNCH_CHECK("bbox_cd_loss_kernel");
-  return ESB_OK;
+  int rc = esb_sum_partial_rows(part, grid, 1, loss_out, 1, s);
+  ESB_CUDA_CALL(esb_scratch_free(part, s));
+  return rc;
 }

@@ -25,7 +25,7 @@ __global__ void sumsq_kernel(const float* __restrict__ g, long long n, float* __
   if (threadIdx.x < 32) {
     float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
     v = esb_warp_sum(v);
-    if (threadIdx.x == 0) atomicAdd(out, v);
+    if (threadIdx.x == 0) out[blockIdx.x] = v;             // one partial per block, summed in block order
   }
 }
 
@@ -74,9 +74,14 @@ extern "C" int esb_grad_clip_coef(const float* grad, long long n, float max_norm
   ESB_CUDA_CALL(cudaMemsetAsync(state, 0, 3 * sizeof(float), stream));
   if (n > 0) {
     int grid = esb_div_up(n, 256 * 4 * 8);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > esb_sm_count() * 8) grid = esb_sm_count() * 8;
     if (grid < 1) grid = 1;
-    sumsq_kernel<<<grid, 256, 0, stream>>>(grad, n, state);
+    float* part = nullptr;
+    ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, (size_t)grid * sizeof(float), stream));
+    sumsq_kernel<<<grid, 256, 0, stream>>>(grad, n, part);
+    int rc = esb_sum_partial_rows(part, grid, 1, state, 0, stream);
+    ESB_CUDA_CALL(esb_scratch_free(part, stream));
+    if (rc != ESB_OK) return rc;
   }
   clip_coef_kernel<<<1, 1, 0, stream>>>(state, max_norm, world_scale);
   ESB_CUDA_LAUNCH_CHECK("esb_grad_clip_coef");

@@ -10,6 +10,7 @@
 // Quirks kept (SURVEY H4): the SUM runs over every view whose nearest pixel is inside the feature map, while the
 // divisor counts only views passing the strict 0<x<w, 0<y<h, depth>0 test in padded-pixel units.
 // HBM-bound: per point 12 B coords + v̄·C·e gathered + C·e written; a warp owns a point, lanes split channels.
+#include <cub/cub.cuh>
 #include "common.cuh"
 
 #define ESB_PAINT_MAX_OPS 8
@@ -137,49 +138,61 @@ __global__ void paint_fwd_kernel(const int* __restrict__ coords, const float* __
   if (lane == 0 && valid_count) valid_count[n] = count;
 }
 
-// dfeat (fp32, same layout as feat) += dout[n] / count for every view whose nearest pixel is inside the map
+// Backward, deterministic: a point's gradient dout[n] / count goes to the nearest pixel of every view that sees it. Pass 1
+// writes one (pixel key, point) pair per (point, view) — key = (b*V + v)*Hf*Wf + pixel, or ~0u for a view that does not see
+// the point; a stable radix sort groups the pairs by pixel with the points of a pixel in index order; pass 2 (one warp per
+// pixel) adds them in that order, so dfeat does not depend on scheduling.
 template <typename T>
-__global__ void paint_bwd_kernel(const int* __restrict__ coords, const float* __restrict__ fpts,
-                                 const int* __restrict__ fbatch, long long N, float voxel_size,
-                                 const EsbPaintMeta* __restrict__ metas, const float* __restrict__ proj, int V,
-                                 const T* __restrict__ dout, int Hf, int Wf, int C, float pad_h, float pad_w,
-                                 float* __restrict__ dfeat) {
+__global__ void paint_bwd_pairs_kernel(const int* __restrict__ coords, const float* __restrict__ fpts,
+                                       const int* __restrict__ fbatch, long long N, float voxel_size,
+                                       const EsbPaintMeta* __restrict__ metas, const float* __restrict__ proj, int V, int Hf,
+                                       int Wf, float pad_h, float pad_w, unsigned* __restrict__ keys, int* __restrict__ pts,
+                                       float* __restrict__ inv_count) {
   const int lane = threadIdx.x & 31;
   const long long n = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
   if (n >= N) return;
   int b; float x, y, z;
   point_of(coords, fpts, fbatch, n, voxel_size, metas, &b, &x, &y, &z);
   const EsbPaintMeta& m = metas[b];
-  // first pass: count valid views
   int count = 0;
-  for (int vb = 0; vb < V; vb += 32) {
-    int v = vb + lane, ok = 0;
-    if (v < V) project(proj + ((long long)b * V + v) * 16, m, x, y, z, pad_h, pad_w, Hf, Wf, &ok);
-    count += __popc(__ballot_sync(0xffffffffu, ok));
-  }
-  if (count == 0) return;
-  float inv = 1.f / (float)count;
-  float g[16];
-#pragma unroll
-  for (int q = 0; q < 16; ++q) {
-    int c = lane + 32 * q;
-    g[q] = c < C ? esb_to_float<T>(dout[n * C + c]) * inv : 0.f;
-  }
   for (int vb = 0; vb < V; vb += 32) {
     int v = vb + lane, pix = -1, ok = 0;
     if (v < V) pix = project(proj + ((long long)b * V + v) * 16, m, x, y, z, pad_h, pad_w, Hf, Wf, &ok);
-    unsigned hit = __ballot_sync(0xffffffffu, pix >= 0);
-    while (hit) {
-      int j = __ffs(hit) - 1;
-      hit &= hit - 1;
-      int pj = __shfl_sync(0xffffffffu, pix, j);
-      float* dst = dfeat + (((long long)b * V + vb + j) * Hf * Wf + pj) * C;
-#pragma unroll
-      for (int q = 0; q < 16; ++q) {
-        int c = lane + 32 * q;
-        if (c < C) atomicAdd(dst + c, g[q]);
-      }
+    count += __popc(__ballot_sync(0xffffffffu, ok));
+    if (v < V) {
+      keys[n * V + v] = pix >= 0 ? (unsigned)(((long long)b * V + v) * Hf * Wf + pix) : ~0u;
+      pts[n * V + v] = (int)n;
     }
+  }
+  if (lane == 0) inv_count[n] = count > 0 ? 1.f / (float)count : 0.f;
+}
+
+template <typename T>
+__global__ void paint_bwd_sum_kernel(const unsigned* __restrict__ keys, const int* __restrict__ pts, long long n_pairs,
+                                     const float* __restrict__ inv_count, const T* __restrict__ dout, int C,
+                                     float* __restrict__ dfeat) {
+  const int lane = threadIdx.x & 31;
+  const long long i = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+  if (i >= n_pairs) return;
+  const unsigned key = keys[i];
+  if (key == ~0u || (i > 0 && keys[i - 1] == key)) return;          // not the first pair of a seen pixel
+  float acc[16];
+#pragma unroll
+  for (int q = 0; q < 16; ++q) acc[q] = 0.f;
+  for (long long j = i; j < n_pairs && keys[j] == key; ++j) {
+    const long long n = pts[j];
+    const float inv = inv_count[n];
+#pragma unroll
+    for (int q = 0; q < 16; ++q) {
+      const int c = lane + 32 * q;
+      if (c < C) acc[q] += esb_to_float<T>(dout[n * C + c]) * inv;
+    }
+  }
+  float* dst = dfeat + (long long)key * C;
+#pragma unroll
+  for (int q = 0; q < 16; ++q) {
+    const int c = lane + 32 * q;
+    if (c < C) dst[c] += acc[q];
   }
 }
 
@@ -207,21 +220,49 @@ extern "C" int esb_paint_fwd(const int* coords, const float* fpts, const int* fb
   return ESB_OK;
 }
 
-// dfeat must be zero-initialised fp32 with the layout of feat.
+// dfeat (fp32, the layout of feat) += d out / d feat; zero-initialised by the caller for a plain gradient.
 extern "C" int esb_paint_bwd(const int* coords, const float* fpts, const int* fbatch, long long N, float voxel_size,
                              const void* metas, const float* proj,
                              int V, const void* dout, int Hf, int Wf, int C, float pad_h, float pad_w, float* dfeat,
-                             int dtype, void* stream) {
+                             int dtype, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   ESB_CHECK_ARG(C >= 1 && C <= 512, "esb_paint_bwd: C must be in [1,512]");
   if (N == 0) return ESB_OK;
-  int grid = esb_div_up(N * 32, 256);
+  const long long n_pairs = N * V;
+  ESB_CHECK_ARG(n_pairs < (1LL << 31), "esb_paint_bwd: too many (point, view) pairs");
+  // pixel keys stay below 2^32 - 1 (the "not seen" marker) for feature maps of fewer than 4G pixels in all
+  size_t temp_bytes = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr,
+                                  (int*)nullptr, (int)n_pairs, 0, 32, stream);
+  const size_t a_pairs = esb_align((size_t)n_pairs * 4);
+  uint8_t* ws = nullptr;
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&ws, 4 * a_pairs + esb_align((size_t)N * 4) + esb_align(temp_bytes), stream));
+  unsigned* keys = (unsigned*)ws;
+  unsigned* keys_s = (unsigned*)(ws + a_pairs);
+  int* pts = (int*)(ws + 2 * a_pairs);
+  int* pts_s = (int*)(ws + 3 * a_pairs);
+  float* inv = (float*)(ws + 4 * a_pairs);
+  void* temp = ws + 4 * a_pairs + esb_align((size_t)N * 4);
+  const int grid = esb_div_up(N * 32, 256), grid2 = esb_div_up(n_pairs * 32, 256);
   if (dtype == ESB_F32)
-    paint_bwd_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(coords, fpts, fbatch, N, voxel_size, (const EsbPaintMeta*)metas, proj,
-                                                                     V, (const float*)dout, Hf, Wf, C, pad_h, pad_w, dfeat);
+    paint_bwd_pairs_kernel<float><<<grid, 256, 0, stream>>>(coords, fpts, fbatch, N, voxel_size, (const EsbPaintMeta*)metas, proj,
+                                                            V, Hf, Wf, pad_h, pad_w, keys, pts, inv);
   else
-    paint_bwd_kernel<__nv_bfloat16><<<grid, 256, 0, (cudaStream_t)stream>>>(
-        coords, fpts, fbatch, N, voxel_size, (const EsbPaintMeta*)metas, proj, V, (const __nv_bfloat16*)dout, Hf, Wf, C, pad_h, pad_w,
-        dfeat);
-  ESB_CUDA_LAUNCH_CHECK("paint_bwd_kernel");
+    paint_bwd_pairs_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(coords, fpts, fbatch, N, voxel_size, (const EsbPaintMeta*)metas,
+                                                                    proj, V, Hf, Wf, pad_h, pad_w, keys, pts, inv);
+  ESB_CUDA_LAUNCH_CHECK("paint_bwd_pairs_kernel");
+  cudaError_t e = cub::DeviceRadixSort::SortPairs(temp, temp_bytes, keys, keys_s, pts, pts_s, (int)n_pairs, 0, 32, stream);
+  if (e != cudaSuccess) {
+    esb_scratch_free(ws, stream);
+    esb_set_error("esb_paint_bwd: sort: %s", cudaGetErrorString(e));
+    return ESB_ECUDA;
+  }
+  if (dtype == ESB_F32)
+    paint_bwd_sum_kernel<float><<<grid2, 256, 0, stream>>>(keys_s, pts_s, n_pairs, inv, (const float*)dout, C, dfeat);
+  else
+    paint_bwd_sum_kernel<__nv_bfloat16><<<grid2, 256, 0, stream>>>(keys_s, pts_s, n_pairs, inv, (const __nv_bfloat16*)dout, C,
+                                                                   dfeat);
+  ESB_CUDA_LAUNCH_CHECK("paint_bwd_sum_kernel");
+  ESB_CUDA_CALL(esb_scratch_free(ws, stream));
   return ESB_OK;
 }

@@ -178,7 +178,8 @@ spconv_wgrad_kernel(const T* __restrict__ x, const T* __restrict__ dy, const int
     }
     __syncthreads();
   }
-  float* dwk = dw + (long long)k * cin * cout;
+  // this split's partial of dW[k]: part[sp][k] (zeroed by the host: splits without pairs leave it untouched)
+  float* dwk = dw + ((long long)sp * gridDim.x / splits + k) * cin * cout;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     int ci = ci0 + ty * 4 + i;
@@ -186,7 +187,7 @@ spconv_wgrad_kernel(const T* __restrict__ x, const T* __restrict__ dy, const int
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       int co = co0 + tx * 4 + j;
-      if (co < cout) atomicAdd(&dwk[(long long)ci * cout + co], acc[i][j]);
+      if (co < cout) dwk[(long long)ci * cout + co] = acc[i][j];
     }
   }
 }
@@ -214,7 +215,8 @@ extern "C" int esb_spconv_fwd(const void* x, const void* w, const int* nbr, void
   return ESB_OK;
 }
 
-// dw (K,cin,cout) fp32, must be zeroed by the caller (the kernel accumulates with atomics over pair splits).
+// dw (K,cin,cout) fp32 += the weight gradient (zeroed by the caller for a plain gradient); the pair splits' partials are
+// added in split order.
 extern "C" int esb_spconv_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out,
                                 const int* k_offsets, float* dw, long long n_pairs_hint, int cin, int cout, int K,
                                 int dtype, void* stream_) {
@@ -222,20 +224,26 @@ extern "C" int esb_spconv_wgrad(const void* x, const void* dy, const int* pair_i
   ESB_CHECK_ARG(cin > 0 && cout > 0 && K > 0, "esb_spconv_wgrad: bad channel/kernel sizes");
   ESB_CHECK_ARG(dtype == ESB_F32 || dtype == ESB_BF16, "esb_spconv_wgrad: dtype must be f32 or bf16");
   int ci_t = esb_div_up(cin, TM), co_t = esb_div_up(cout, TN);
-  // aim for ~4 CTAs/SM over 148 SMs, but keep >= 256 pairs per split
+  // aim for ~4 CTAs/SM over the SMs, but keep >= 256 pairs per split
   long long per_k = n_pairs_hint / K + 1;
-  int splits = (int)(592 / ((long long)K * ci_t * co_t));
+  int splits = (int)(4LL * esb_sm_count() / ((long long)K * ci_t * co_t));
   int max_by_pairs = (int)(per_k / 256) + 1;
   if (splits > max_by_pairs) splits = max_by_pairs;
   if (splits < 1) splits = 1;
   if (splits > 64) splits = 64;
   dim3 grid(K * splits, ci_t, co_t);
+  const long long width = (long long)K * cin * cout;
+  float* part = nullptr;
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, sizeof(float) * splits * width, stream));
+  ESB_CUDA_CALL(cudaMemsetAsync(part, 0, sizeof(float) * splits * width, stream));
   if (dtype == ESB_F32)
     spconv_wgrad_kernel<float><<<grid, 256, 0, stream>>>((const float*)x, (const float*)dy, pair_in, pair_out,
-                                                          k_offsets, dw, cin, cout, splits);
+                                                          k_offsets, part, cin, cout, splits);
   else
     spconv_wgrad_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)dy,
-                                                                  pair_in, pair_out, k_offsets, dw, cin, cout, splits);
+                                                                  pair_in, pair_out, k_offsets, part, cin, cout, splits);
   ESB_CUDA_LAUNCH_CHECK("spconv_wgrad_kernel");
-  return ESB_OK;
+  int rc = esb_sum_partial_rows(part, splits, width, dw, 1, stream);
+  ESB_CUDA_CALL(esb_scratch_free(part, stream));
+  return rc;
 }

@@ -48,7 +48,8 @@ __device__ __forceinline__ int seg_end(const int* __restrict__ seg_off, int s, i
 }
 
 // ---------------- segmented column statistics ----------------
-// pass 1: sum over rows of each segment -> out[s][c]; pass 2 (centered): sum (x-mean)^2.
+// pass 1: sum over rows of each segment; pass 2 (centered): sum (x-mean)^2. Block (bx, s, cz) writes its partial to
+// out[bx][s][c]; esb_sum_partial_rows adds the row blocks in order.
 template <typename T, int MODE>  // MODE 0: sum x ; 1: sum (x - mean[s][c])^2
 __global__ void seg_colstat_kernel(const T* __restrict__ x, const int* __restrict__ seg_off, const float* __restrict__ mean,
                                    float* __restrict__ out, int C, int rows_per_block, int n_total) {
@@ -72,11 +73,11 @@ __global__ void seg_colstat_kernel(const T* __restrict__ x, const int* __restric
   }
   red[threadIdx.y][threadIdx.x] = acc;
   __syncthreads();
-  if (threadIdx.y == 0 && c < C && r_beg < r_end) {
+  if (threadIdx.y == 0 && c < C) {
     float t = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) t += red[j][threadIdx.x];
-    atomicAdd(&out[s * C + c], t);
+    out[((long long)blockIdx.x * gridDim.y + s) * C + c] = t;
   }
 }
 
@@ -223,7 +224,7 @@ __global__ void norm_bwd_apply_vec8_kernel(const T* __restrict__ x, const T* __r
   if (dres) store8<T>(dres + t * 8, gv);
 }
 
-// backward reduce: sg[s][c] = sum g ; sgx[s][c] = sum g * xhat, with g = dy * act'(y)
+// backward reduce: sg[s][c] = sum g ; sgx[s][c] = sum g * xhat, with g = dy * act'(y); partials per row block as above
 template <typename T>
 __global__ void norm_bwd_reduce_kernel(const T* __restrict__ x, const T* __restrict__ y, const T* __restrict__ dy,
                                        const int* __restrict__ seg_off, const float* __restrict__ mean,
@@ -249,15 +250,15 @@ __global__ void norm_bwd_reduce_kernel(const T* __restrict__ x, const T* __restr
   red0[threadIdx.y][threadIdx.x] = a0;
   red1[threadIdx.y][threadIdx.x] = a1;
   __syncthreads();
-  if (threadIdx.y == 0 && c < C && r_beg < r_end) {
+  if (threadIdx.y == 0 && c < C) {
     float t0 = 0.f, t1 = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       t0 += red0[j][threadIdx.x];
       t1 += red1[j][threadIdx.x];
     }
-    atomicAdd(&sg[s * C + c], t0);
-    atomicAdd(&sgx[s * C + c], t1);
+    sg[((long long)blockIdx.x * gridDim.y + s) * C + c] = t0;
+    sgx[((long long)blockIdx.x * gridDim.y + s) * C + c] = t1;
   }
 }
 
@@ -354,12 +355,8 @@ __global__ void act_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ y
 // catastrophic cancellation a raw single-pass variance has when |mean| >> std), accumulated per block in shared memory and
 // added to stats[0] (sum v), stats[1] (sum v^2). The apply kernel turns them into mean / rstd on the fly.
 template <typename T>
-__global__ void bn_stats_kernel(const T* __restrict__ x, long long N, int C, int rows_per_block, float* __restrict__ stats) {
-  extern __shared__ float sh[];                    // [2][C]
-  float* s_sum = sh;
-  float* s_sq = sh + C;
-  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) sh[i] = 0.f;
-  __syncthreads();
+__global__ void bn_stats_kernel(const T* __restrict__ x, long long N, int C, int rows_per_block, float* __restrict__ part) {
+  extern __shared__ float sh[];                    // [rstep][2][C]: one slot per row lane, summed in lane order
   const int tpr = C / 8;                           // threads per row (16-byte pieces)
   const int c = (threadIdx.x % tpr) * 8;
   const int rsub = threadIdx.x / tpr, rstep = blockDim.x / tpr;
@@ -382,14 +379,17 @@ __global__ void bn_stats_kernel(const T* __restrict__ x, long long N, int C, int
     }
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
-      atomicAdd(&s_sum[c + e], sum[e]);
-      atomicAdd(&s_sq[c + e], sq[e]);
+      sh[(2 * rsub) * C + c + e] = sum[e];
+      sh[(2 * rsub + 1) * C + c + e] = sq[e];
     }
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < C; i += blockDim.x) {
-    atomicAdd(&stats[i], s_sum[i]);
-    atomicAdd(&stats[C + i], s_sq[i]);
+  // this block's partial: part[blockIdx][0 .. C) = sum, [C .. 2C) = sum of squares
+  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
+    const int k = i < C ? 0 : 1, ci = i < C ? i : i - C;
+    float t = 0.f;
+    for (int r = 0; r < rstep; ++r) t += sh[(2 * r + k) * C + ci];
+    part[(long long)blockIdx.x * 2 * C + i] = t;
   }
 }
 
@@ -512,10 +512,15 @@ extern "C" int esb_norm_fwd(const void* x, const void* res, const int* seg_off, 
   const int rpb = 256;
   dim3 grid(esb_div_up(max_seg_rows > 0 ? max_seg_rows : 1, rpb), S, esb_div_up(C, 32)), block(32, 8);
   int fin = esb_div_up(S * C, 256);
+  float* part = nullptr;
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, sizeof(float) * grid.x * S * C, stream));
+  int rc = ESB_OK;
   DISPATCH_T(dtype, {
-    seg_colstat_kernel<T, 0><<<grid, block, 0, stream>>>((const T*)x, seg_off, nullptr, mean, C, rpb, (int)N);
+    seg_colstat_kernel<T, 0><<<grid, block, 0, stream>>>((const T*)x, seg_off, nullptr, part, C, rpb, (int)N);
+    rc = esb_sum_partial_rows(part, (int)grid.x, (long long)S * C, mean, 0, stream);
     seg_finalize_mean_kernel<<<fin, 256, 0, stream>>>(mean, seg_off, S, C, (int)N);
-    seg_colstat_kernel<T, 1><<<grid, block, 0, stream>>>((const T*)x, seg_off, mean, rstd, C, rpb, (int)N);
+    seg_colstat_kernel<T, 1><<<grid, block, 0, stream>>>((const T*)x, seg_off, mean, part, C, rpb, (int)N);
+    if (rc == ESB_OK) rc = esb_sum_partial_rows(part, (int)grid.x, (long long)S * C, rstd, 0, stream);
     seg_finalize_rstd_kernel<<<fin, 256, 0, stream>>>(mean, rstd, seg_off, S, C, eps, running_mean, running_var, momentum,
                                                       (int)N);
     if (C % 8 == 0)
@@ -525,6 +530,8 @@ extern "C" int esb_norm_fwd(const void* x, const void* res, const int* seg_off, 
       norm_apply_kernel<T><<<esb_div_up(N * C, 256), 256, 0, stream>>>((const T*)x, (const T*)res, row_seg, mean, rstd,
                                                                        gamma, beta, (T*)y, N, C, act);
   });
+  ESB_CUDA_CALL(esb_scratch_free(part, stream));
+  if (rc != ESB_OK) return rc;
   ESB_CUDA_LAUNCH_CHECK("esb_norm_fwd");
   return ESB_OK;
 }
@@ -554,9 +561,15 @@ extern "C" int esb_norm_bwd(const void* x, const void* y, const void* dy, const 
   if (N == 0) return ESB_OK;
   const int rpb = 256;
   dim3 grid(esb_div_up(max_seg_rows > 0 ? max_seg_rows : 1, rpb), S, esb_div_up(C, 32)), block(32, 8);
+  const long long width = (long long)S * C;
+  float* part = nullptr;
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, sizeof(float) * 2 * grid.x * width, stream));
+  int rc = ESB_OK;
   DISPATCH_T(dtype, {
     norm_bwd_reduce_kernel<T><<<grid, block, 0, stream>>>((const T*)x, (const T*)y, (const T*)dy, seg_off, mean, rstd,
-                                                          sg, sgx, C, rpb, act, (int)N);
+                                                          part, part + grid.x * width, C, rpb, act, (int)N);
+    rc = esb_sum_partial_rows(part, (int)grid.x, width, sg, 1, stream);
+    if (rc == ESB_OK) rc = esb_sum_partial_rows(part + grid.x * width, (int)grid.x, width, sgx, 1, stream);
     if (C % 8 == 0)
       norm_bwd_apply_vec8_kernel<T><<<esb_div_up(N * (C / 8), 256), 256, 0, stream>>>(
           (const T*)x, (const T*)y, (const T*)dy, row_seg, seg_off, mean, rstd, gamma, sg, sgx, (T*)dx, (T*)dres, N,
@@ -565,6 +578,8 @@ extern "C" int esb_norm_bwd(const void* x, const void* y, const void* dy, const 
       norm_bwd_apply_kernel<T><<<esb_div_up(N * C, 256), 256, 0, stream>>>(
           (const T*)x, (const T*)y, (const T*)dy, row_seg, seg_off, mean, rstd, gamma, sg, sgx, (T*)dx, (T*)dres, N, C, act);
   });
+  ESB_CUDA_CALL(esb_scratch_free(part, stream));
+  if (rc != ESB_OK) return rc;
   ESB_CUDA_LAUNCH_CHECK("esb_norm_bwd");
   return ESB_OK;
 }
@@ -620,12 +635,18 @@ extern "C" int esb_batchnorm_fwd_fused(const void* x, const void* res, long long
   ESB_CHECK_ARG(C % 8 == 0 && C >= 8 && C <= 2048, "esb_batchnorm_fwd_fused: C must be a multiple of 8 in [8, 2048]");
   ESB_CUDA_CALL(cudaMemsetAsync(stats, 0, sizeof(float) * 2 * C, stream));
   if (N == 0) return ESB_OK;
-  long long rpb = (N + 295) / 296;
+  long long rpb = (N + 2 * esb_sm_count() - 1) / (2 * esb_sm_count());
   if (rpb < 64) rpb = 64;
   const int grid_a = esb_div_up(N, rpb);
   const long long n_vec = N * (C / 8);
-  DISPATCH_T(dtype, (bn_stats_kernel<T><<<grid_a, 256, 2 * C * sizeof(float), stream>>>((const T*)x, N, C, (int)rpb, stats)));
+  const int rstep = 256 / (C / 8);
+  float* part = nullptr;
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, sizeof(float) * 2 * C * grid_a, stream));
+  DISPATCH_T(dtype, (bn_stats_kernel<T><<<grid_a, 256, 2 * rstep * C * sizeof(float), stream>>>((const T*)x, N, C, (int)rpb, part)));
   ESB_CUDA_LAUNCH_CHECK("bn_stats_kernel");
+  int rc = esb_sum_partial_rows(part, grid_a, 2LL * C, stats, 0, stream);
+  ESB_CUDA_CALL(esb_scratch_free(part, stream));
+  if (rc != ESB_OK) return rc;
   DISPATCH_T(dtype, (bn_apply_fused_kernel<T><<<esb_div_up(n_vec, 256), 256, 0, stream>>>(
                         (const T*)x, (const T*)res, N, C, gamma, beta, eps, running_mean, running_var, momentum, act, stats,
                         (T*)y)));
@@ -733,7 +754,8 @@ __global__ void __launch_bounds__(256) head_split_bwd_kernel(const __nv_bfloat16
 
 static int head_split_grid(long long N) {
   long long g = esb_div_up(N, 8);                    // 8 warps (rows) per block
-  return (int)(g < 148 * 4 ? g : 148 * 4);
+  const long long cap = 4LL * esb_sm_count();
+  return (int)(g < cap ? g : cap);
 }
 
 extern "C" int esb_head_split_fwd(const void* out, const float* bias, const float* scale, long long N, int W, int n_cls,

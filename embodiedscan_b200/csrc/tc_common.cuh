@@ -1,8 +1,9 @@
-// esb200 — tcgen05 / TMEM / mbarrier / cp.async / TMA primitives shared by every tensor-core kernel of the library
+// esb200 — wgmma / mbarrier / cp.async / TMA primitives shared by every tensor-core kernel of the library
 // (spconv_tc.cu, conv2d_tc.cu, conv_tma.cu, attn_tc.cu): ONE copy of the descriptor encoders.
 #pragma once
 #include <cuda.h>            // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint)
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace esb_tc {
 
@@ -41,76 +42,62 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- warpgroup MMA (wgmma) ------------------------------------------------------------------------------------------
+// A 128-row accumulator tile is owned by two consumer warpgroups, 64 rows each (wgmma is m64); the fragment lives in
+// registers and is written once per tile to a row-major fp32 image in shared memory (acc_store), which the epilogue
+// threads read row by row (img_ld) — thread = tile row, as the epilogues of these kernels are written.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
+template <int R>
+__device__ __forceinline__ void acc_zero(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) d[i] = 0.f;
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// m64nN fp32 fragment layout: element i of thread t (0..127 in the warpgroup) is row 16*(t/32) + (t%32)/4 + 8*((i/2)%2),
+// column 8*(i/4) + 2*(t%4) + i%2.
+template <int N>
+__device__ __forceinline__ void acc_store(const float* d, float* img, int pitch, int row0, int t) {
+  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    *reinterpret_cast<float2*>(img + r * pitch + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(img + (r + 8) * pitch + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
 }
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 | LBO>>4 <<16 | SBO>>4 <<32 | version 1 <<46 |
-// layout type <<61 (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         (1ull << 46) | (2ull << 61);
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D fp32, A/B bf16, majors, N>>3, M>>4
-__device__ __forceinline__ uint32_t make_idesc(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t v[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-      "%24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t v[32]) {      // 16 columns into v[0..15]
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// NCOL consecutive fp32 of row `row` starting at column `col` (16-byte aligned) into v[0..NCOL-1]
+template <int NCOL>
+__device__ __forceinline__ void img_ld(const float* img, int pitch, int row, int col, uint32_t v[32]) {
+#pragma unroll
+  for (int q = 0; q < NCOL / 4; ++q) {
+    const float4 f = *reinterpret_cast<const float4*>(img + row * pitch + col + 4 * q);
+    v[4 * q] = __float_as_uint(f.x); v[4 * q + 1] = __float_as_uint(f.y);
+    v[4 * q + 2] = __float_as_uint(f.z); v[4 * q + 3] = __float_as_uint(f.w);
+  }
 }
 __device__ __forceinline__ uint32_t pack_bf16(uint32_t lo_f32_bits, uint32_t hi_f32_bits) {
   __nv_bfloat162 h = __floats2bfloat162_rn(__uint_as_float(lo_f32_bits), __uint_as_float(hi_f32_bits));
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// ---- generalised shared-memory descriptor: layout_type 0 none, 2 SWIZZLE_128B, 4 SWIZZLE_64B, 6 SWIZZLE_32B -----------
+// ---- shared-memory matrix descriptor (wgmma): start>>4 | LBO>>4 <<16 | SBO>>4 <<32 | layout type <<62 ----------------
+constexpr uint32_t SW128 = 1, SW64 = 2, SW32 = 3;     // layout types: 128B / 64B / 32B swizzle
 __device__ __forceinline__ uint64_t make_desc_sw(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type) {
   return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         (1ull << 46) | ((uint64_t)layout_type << 61);
+         ((uint64_t)layout_type << 62);
 }
-// UMMA layout type of a row of `row_bytes` bytes (32 / 64 / 128): one swizzle span per row
-__host__ __device__ __forceinline__ uint32_t umma_layout_of(int row_bytes) { return row_bytes >= 128 ? 2u : row_bytes == 64 ? 4u : 6u; }
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return make_desc_sw(smem_addr, lbo_bytes, sbo_bytes, SW128);
+}
+// layout type of a row of `row_bytes` bytes (32 / 64 / 128): one swizzle span per row
+__host__ __device__ __forceinline__ uint32_t mma_layout_of(int row_bytes) { return row_bytes >= 128 ? SW128 : row_bytes == 64 ? SW64 : SW32; }
 
 // ---- TMA (cp.async.bulk.tensor) -------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -135,12 +122,6 @@ __device__ __forceinline__ void tma_load_5d(const CUtensorMap* m, uint64_t* bar,
                                             int c4) {
   asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
                ::"r"(dst), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-// four rows (r0..r3) of a 2-D tensor, `box inner` columns starting at column c0; rows out of range are zero-filled
-__device__ __forceinline__ void tma_gather4(const CUtensorMap* m, uint64_t* bar, uint32_t dst, int c0, int r0, int r1, int r2,
-                                            int r3) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-               ::"r"(dst), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
 }
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];"

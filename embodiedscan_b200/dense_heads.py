@@ -35,7 +35,7 @@ class Scale(nn.Module):
 
 def head_epilogue_backend() -> str:
     """'lib' (default): the ATen slice / exp / clamp / cat chain after the head GEMM. ESB200_HEAD_EPILOGUE=own switches to the
-    fused kernel pair (esb_head_split_fwd / _bwd): green against that chain in tests/test_kernels_gpu.py on a B200, but the
+    fused kernel pair (esb_head_split_fwd / _bwd): checked against that chain in tests/test_kernels_gpu.py, but the
     round's GPU time ran out before the whole training step was re-validated with it, so it is not the default yet."""
     import os
     return os.environ.get('ESB200_HEAD_EPILOGUE', 'lib')

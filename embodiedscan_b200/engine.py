@@ -179,7 +179,7 @@ class OptimWrapper:
         self.max_run_ahead = max_run_ahead
         self._step_events = []
         # The interpreter's automatic cyclic collector pauses a step for 70-260 ms whenever a generation-1 pass falls into
-        # it (measured on the B200 box: 4 passes = 4 stalls per 40 steps, none with the collector off; on N ranks the pauses
+        # it (4 passes = 4 stalls per 40 steps, none with the collector off; on N ranks the pauses
         # land on different steps of different ranks and every rank waits for the slowest). Like other synchronous
         # data-parallel trainers the wrapper therefore takes the collector over: automatic collection off, one young-generation
         # pass every `gc_interval` optimiser steps, at the same step on every rank, issued while the device is still busy

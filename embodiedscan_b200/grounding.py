@@ -5,7 +5,7 @@ names: ``SparseFeatureFusion3DGrounder`` (embodiedscan/models/detectors/sparse_f
 ``ContrastiveEmbed`` (models/dense_heads/grounding_head.py:22-824), ``HungarianAssigner3D``
 (models/task_modules/assigners/hungarian_assigner.py:17-138) and the match costs (models/losses/match_cost.py).
 
-What is B200-native here:
+What is H100-native here:
 * the front half (voxel hashing, MinkResNet, painting, the pruned sparse FPN) runs in libesb200.so like the detector;
 * target assignment is ONE device launch for all decoder layers x samples (``esb_hungarian_batch``) fed by batched
   cost tensors and the exact 9-DoF IoU kernel (``esb_box3d_overlap``) — the reference does 7 x batch D2H copies,
@@ -122,7 +122,7 @@ class PositionEmbeddingLearned(nn.Module):
 
 
 class _FlashAttention(torch.autograd.Function):
-    """softmax(q k^T * scale + key padding) v for 32-channel heads on the library's tcgen05 flash-attention tiles
+    """softmax(q k^T * scale + key padding) v for 32-channel heads on the library's wgmma flash-attention tiles
     (csrc/attn_tc.cu), forward and backward. q (B,H,Lq,32), k / v (B,H,Lk,32) bf16 contiguous; key_pad (B,Lk) bool or None."""
 
     @staticmethod
@@ -184,7 +184,7 @@ class MultiheadAttention(nn.Module):
         E, H = self.embed_dims, self.num_heads
         if (query.is_cuda and attn_mask is None and E // H == 32 and torch.is_autocast_enabled()
                 and torch.get_autocast_gpu_dtype() == torch.bfloat16 and os.environ.get('ESB200_ATTN', 'own') == 'own'):
-            # the projections are plain library GEMMs; the attention core runs on the library's tcgen05 flash tiles
+            # the projections are plain library GEMMs; the attention core runs on the library's wgmma flash tiles
             W, bias = self.attn.in_proj_weight, self.attn.in_proj_bias
             B, Lq, Lk = query.shape[0], query.shape[1], key.shape[1]
             q = F.linear(query, W[:E], bias[:E]).view(B, Lq, H, 32).transpose(1, 2)

@@ -7,7 +7,7 @@ SurroundOcc losses (models/losses/occ_loss.py:7-141).
 Shares the front half with the detector — voxel hashing, MinkResNet34 and the point-painting kernel (here on the prior
 grid's fp32 voxel centres) all run in libesb200.so. The dense Conv3d FPN is the one tensor-core-bound stage of the named
 configs (~4 TFLOP/scan); this round it is evaluated by the library convolution (cuDNN) in channels-last-3d bf16 — the
-tcgen05 implicit-GEMM Conv3d is listed in DESIGN.md §7.
+wgmma implicit-GEMM Conv3d is listed in DESIGN.md §7.
 """
 from typing import List, Optional
 
@@ -82,7 +82,7 @@ class _ConvOnly(nn.Module):
 
 
 def _tma3d_ok(x, conv) -> bool:
-    """The dense 3-D stack runs on the library's TMA + tcgen05 kernels (csrc/conv_tma.cu, rank-5 tensor maps) when the
+    """The dense 3-D stack runs on the library's TMA + wgmma kernels (csrc/conv_tma.cu, rank-5 tensor maps) when the
     activations are bf16 on the GPU and the channel counts tile (16, 32, multiples of 64; outputs a power of two <= 256 or a
     multiple of 256); anything else (fp32 parity arithmetic, toy widths) stays on the library convolution."""
     import os

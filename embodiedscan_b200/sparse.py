@@ -24,15 +24,9 @@ from ._ffi import call, ptr, query, stream
 
 ACT_NONE, ACT_RELU, ACT_ELU = 0, 1, 2
 
-# bf16 sparse convolutions run on tcgen05 tensor cores when the channel counts tile (multiples of 64)
+# bf16 sparse convolutions run on the wgmma tensor-core kernels when the channel counts tile (multiples of 64)
 USE_TENSOR_CORES = True
 USE_TC_WGRAD = True
-
-
-def spconv_backend() -> str:
-    """'tma' (operands fed by cp.async.bulk.tensor: gather4 rows + tiled filter boxes, csrc/spconv_tma.cu) or 'tc' (the
-    round-1 cp.async gather, csrc/spconv_tc.cu). ESB200_SPCONV overrides."""
-    return os.environ.get('ESB200_SPCONV', 'tc')
 
 # bench.py switches this on to time every sparse-conv launch with CUDA events on the launching stream
 CONV_PROFILE = {'enabled': False, 'records': []}
@@ -289,18 +283,14 @@ class _SparseConv(torch.autograd.Function):
         w = bf16_operand(weight) if x.dtype == torch.bfloat16 else weight.detach().to(x.dtype).contiguous()
         y = torch.empty((kmap.n_out, cout), dtype=x.dtype, device=x.device)
         tc = USE_TENSOR_CORES and x.dtype == torch.bfloat16 and cin % 64 == 0 and cout % 64 == 0
-        tma = tc and spconv_backend() == 'tma'
-        if tma:  # same operands, every tile moved by TMA
-            _timed_conv_call('fwd', kmap, cin, cout, x.dtype, 'esb_spconv_tma_fwd', ptr(x), ptr(w), ptr(kmap.nbr_out),
-                             ptr(kmap.tile_masks('out')), ptr(y), kmap.n_in, kmap.n_out, cin, cout, K, 1, stream())
-        elif tc:   # the stored (K,cin,cout) kernel is the MN-major B operand: no transpose copy
+        if tc:   # the stored (K,cin,cout) kernel is the MN-major B operand: no transpose copy
             _timed_conv_call('fwd', kmap, cin, cout, x.dtype, 'esb_spconv_tc_fwd', ptr(x), ptr(w), ptr(kmap.nbr_out),
                              ptr(kmap.tile_masks('out')), ptr(y), kmap.n_out, cin, cout, K, 1, stream())
         else:
             _timed_conv_call('fwd', kmap, cin, cout, x.dtype, 'esb_spconv_fwd', ptr(x), ptr(w), ptr(kmap.nbr_out),
                              ptr(y), kmap.n_out, cin, cout, K, 0, 0, _ffi.dtype_code(x.dtype), stream())
         ctx.save_for_backward(x, w)
-        ctx.kmap, ctx.cin, ctx.cout, ctx.wshape, ctx.tc, ctx.weight, ctx.tma = kmap, cin, cout, weight.shape, tc, weight, tma
+        ctx.kmap, ctx.cin, ctx.cout, ctx.wshape, ctx.tc, ctx.weight = kmap, cin, cout, weight.shape, tc, weight
         if ctx.needs_input_grad[1]:
             _count_use(weight)
         return y
@@ -315,10 +305,7 @@ class _SparseConv(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dx = torch.empty((kmap.n_in, cin), dtype=x.dtype, device=x.device)
             # dgrad = the forward kernel on the input-stationary map with W read transposed
-            if ctx.tma:
-                _timed_conv_call('dgrad', kmap, cout, cin, x.dtype, 'esb_spconv_tma_fwd', ptr(dy), ptr(w), ptr(kmap.nbr_in),
-                                 ptr(kmap.tile_masks('in')), ptr(dx), kmap.n_out, kmap.n_in, cout, cin, kmap.K, 0, stream())
-            elif ctx.tc:   # (K,cin,cout) already is the K-major B operand of the transposed problem
+            if ctx.tc:   # (K,cin,cout) already is the K-major B operand of the transposed problem
                 _timed_conv_call('dgrad', kmap, cout, cin, x.dtype, 'esb_spconv_tc_fwd', ptr(dy), ptr(w), ptr(kmap.nbr_in),
                                  ptr(kmap.tile_masks('in')), ptr(dx), kmap.n_in, cout, cin, kmap.K, 0, stream())
             else:
@@ -330,10 +317,7 @@ class _SparseConv(torch.autograd.Function):
             direct = getattr(weight, '_esb_grad_direct', False) and weight.grad is not None
             # arena parameters: the kernel accumulates straight into the flat gradient buffer (no zeros + add_ pass)
             dw = weight.grad if direct else torch.zeros((kmap.K, cin, cout), dtype=torch.float32, device=x.device)
-            if ctx.tma and USE_TC_WGRAD:
-                _timed_conv_call('wgrad', kmap, cin, cout, x.dtype, 'esb_spconv_tma_wgrad', ptr(x), ptr(dy), ptr(pin),
-                                 ptr(pout), ptr(koff), ptr(dw), kmap.n_in, kmap.n_out, tot, cin, cout, kmap.K, stream())
-            elif ctx.tc and USE_TC_WGRAD:
+            if ctx.tc and USE_TC_WGRAD:
                 _timed_conv_call('wgrad', kmap, cin, cout, x.dtype, 'esb_spconv_tc_wgrad', ptr(x), ptr(dy), ptr(pin),
                                  ptr(pout), ptr(koff), ptr(dw), tot, cin, cout, kmap.K, stream())
             else:
@@ -399,10 +383,7 @@ class _RowsGemmTC(torch.autograd.Function):
         cout = w.shape[1]
         y = torch.empty((N, cout), dtype=torch.bfloat16, device=x.device)
         ar, masks, koff = _identity_map(N, x.device)
-        ctx.tma = spconv_backend() == 'tma'
-        if N and ctx.tma:
-            call('esb_spconv_tma_fwd', ptr(x), ptr(w), ptr(ar), ptr(masks), ptr(y), N, N, cin, cout, 1, 1, stream())
-        elif N:
+        if N:
             call('esb_spconv_tc_fwd', ptr(x), ptr(w), ptr(ar), ptr(masks), ptr(y), N, cin, cout, 1, 1, stream())
         ctx.save_for_backward(x, w)
         return y
@@ -417,16 +398,11 @@ class _RowsGemmTC(torch.autograd.Function):
         dx = dw = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
-            if N and ctx.tma:
-                call('esb_spconv_tma_fwd', ptr(dy), ptr(w), ptr(ar), ptr(masks), ptr(dx), N, N, cout, cin, 1, 0, stream())
-            elif N:
+            if N:
                 call('esb_spconv_tc_fwd', ptr(dy), ptr(w), ptr(ar), ptr(masks), ptr(dx), N, cout, cin, 1, 0, stream())
         if ctx.needs_input_grad[1]:
             dw = torch.zeros((cin, cout), dtype=torch.float32, device=x.device)
-            if N and ctx.tma:
-                call('esb_spconv_tma_wgrad', ptr(x), ptr(dy), ptr(ar), ptr(ar), ptr(koff), ptr(dw), N, N, N, cin, cout, 1,
-                     stream())
-            elif N:
+            if N:
                 call('esb_spconv_tc_wgrad', ptr(x), ptr(dy), ptr(ar), ptr(ar), ptr(koff), ptr(dw), N, cin, cout, 1, stream())
         return dx, dw
 

@@ -1,12 +1,14 @@
-/* esb200.h — C ABI of libesb200.so, the sm_100a kernel library behind the EmbodiedScan hot path.
+/* esb200.h — C ABI of libesb200.so, the sm_90a kernel library behind the EmbodiedScan hot path.
  *
  * The reference (OpenRobotLab/EmbodiedScan) has no FFI of its own: its kernels live in MinkowskiEngine, mmcv._ext and
  * pytorch3d._C. Each entry point below names the reference call site / upstream operator it replaces.
  *
  * Conventions
  *  - plain pointers and sizes only; all pointers are DEVICE pointers unless the name ends in _host.
- *  - the caller owns every buffer (inputs, outputs, workspace); the library never allocates device memory and
- *    keeps no mutable global state. `*_workspace_bytes` returns the scratch size of the paired call.
+ *  - the caller owns every buffer it passes (inputs, outputs, workspace); `*_workspace_bytes` returns the scratch size of
+ *    the paired call. The one memory the library takes itself is the stream-ordered scratch of its deterministic
+ *    reductions (per-block partial sums, added in a fixed order instead of with float atomics): it comes from one
+ *    library-owned memory pool per device, created on first use, and is freed on the same stream within the call.
  *  - every call is asynchronous on `stream` (a cudaStream_t passed as void*), no implicit synchronisation.
  *    Data-dependent output sizes are written to a device int32 the caller reads after synchronising.
  *  - return 0 on success, negative ESB_E* otherwise; esb_last_error() gives a thread-local message.
@@ -62,7 +64,7 @@ int esb_spconv_fwd(const void* x, const void* w, const int* nbr, void* y, long l
 int esb_spconv_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out, const int* k_offsets,
                      float* dw, long long n_pairs_hint, int cin, int cout, int K, int dtype, void* stream);
 
-/* bf16 tensor-core (tcgen05/TMEM) path of the same operator; masks from esb_kmap_tile_masks;
+/* bf16 tensor-core (wgmma) path of the same operator; masks from esb_kmap_tile_masks;
  * w_layout 0: w (K,cout,cin), 1: w (K,cin,cout) — forward and dgrad read the SAME stored bf16 kernel, no transpose */
 int esb_kmap_tile_masks(const int* nbr, int K, long long n, unsigned* masks, void* stream);
 int esb_spconv_tc_fwd(const void* x, const void* wt, const int* nbr, const unsigned* masks, void* y, long long n_out,
@@ -107,9 +109,9 @@ int esb_act_bwd(const void* dy, const void* y, void* dx, long long n, int act, i
  * row gathers of its backward. C % 8 == 0. */
 int esb_gather2_rows(const void* a, const int* ia, long long na, const void* b, const int* ib, void* out, long long n, int C,
                      int dtype, void* stream);
-/* cp.async-gather baseline of the TMA kernels below (validated on the B200; csrc/conv2d_tc.cu): the folded conv+BN(+residual)(+ReLU) block of the per-view 2D
+/* cp.async-gather baseline of the TMA kernels below (csrc/conv2d_tc.cu): the folded conv+BN(+residual)(+ReLU) block of the per-view 2D
  * ResNet (mmdet.ResNet called at embodiedscan/models/detectors/sparse_featfusion_single_stage.py:130-136) as ONE
- * tcgen05 implicit GEMM. x (n_img,H,W,cin) bf16 NHWC; w_ohwi (cout, r_pad) bf16 = the filter in (ky,kx,ci) order,
+ * wgmma implicit GEMM. x (n_img,H,W,cin) bf16 NHWC; w_ohwi (cout, r_pad) bf16 = the filter in (ky,kx,ci) order,
  * each row zero padded from kh*kw*cin to r_pad (multiple of 64); bias (cout) fp32 or NULL; residual / y
  * (n_img,Ho,Wo,cout) bf16 NHWC, residual may be NULL. cin % 8 == 0, cout % 8 == 0. */
 int esb_conv2d_tc_fwd(const void* x, const void* w_ohwi, const float* bias, const void* residual, void* y, int n_img,
@@ -124,25 +126,16 @@ int esb_conv2d_tc_dgrad(const void* dy, const void* w_ihwo, void* dx, int n_img,
  * zeroed by the caller, row r = (ky,kx,ci): dW[co,ci,ky,kx] = dw_t[(ky*kw+kx)*cin+ci, co]. */
 int esb_conv2d_tc_wgrad(const void* x, const void* dy, float* dw_t, int n_img, int H, int W, int cin, int cout, int kh,
                         int kw, int stride, int pad, void* stream);
-/* TMA-fed variants of the two tensor-core sparse-conv entry points (csrc/spconv_tma.cu): gathered rows arrive through
- * cp.async.bulk.tensor tile::gather4 (missing neighbours = out-of-bounds rows = zeros), filter tiles through tiled TMA boxes,
- * forward/dgrad CTAs own 256 output rows per filter stage when the grid allows. Same arguments as esb_spconv_tc_fwd /
- * esb_spconv_tc_wgrad plus the row counts of the gathered tensors (the extents of their tensor maps). */
-int esb_spconv_tma_fwd(const void* x, const void* w, const int* nbr, const unsigned* masks, void* y, long long n_in,
-                       long long n_out, int cin, int cout, int K, int w_layout, void* stream);
-int esb_spconv_tma_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out, const int* k_offsets,
-                         float* dw, long long n_in, long long n_out, long long n_pairs_hint, int cin, int cout, int K,
-                         void* stream);
-/* The per-view 2D backbone's convolution as a persistent TMA + tcgen05 implicit GEMM (csrc/conv_tma.cu): activations,
+/* The per-view 2D backbone's convolution as a persistent TMA + wgmma implicit GEMM (csrc/conv_tma.cu): activations,
  * filter and output move with cp.async.bulk.tensor tiles (zero padding = TMA out-of-bounds fill, stride = tensor-map element
- * strides), accumulators live in TMEM, bias + residual + ReLU are fused into the epilogue. Replaces the cuDNN call behind
+ * strides), accumulators live in registers, bias + residual + ReLU are fused into the epilogue. Replaces the cuDNN call behind
  * mmdet.ResNet (embodiedscan/models/detectors/sparse_featfusion_single_stage.py:130-136). x (n_img,H,W,cin) bf16 NHWC;
  * w_ohwi (cout,kh,kw,cin) bf16; bias (cout) fp32 or NULL; residual / y (n_img,Ho,Wo,cout) bf16 NHWC, residual may be NULL.
  * cin, cout in {16, 32, 64, 128, 256, 512, ...}. */
 int esb_conv2d_tma_fwd(const void* x, const void* w_ohwi, const float* bias, const void* residual, void* y, int n_img,
                        int H, int W, int cin, int cout, int kh, int kw, int stride, int pad, int relu, void* stream);
-/* Weight gradient, TMA-fed (pixels = reduction dimension, both operands arrive as [pixel][channel] boxes = MN-major tcgen05
- * operands): dw_t (kh*kw*cin, cout) fp32, ZEROED BY THE CALLER, dW[co,ci,ky,kx] = dw_t[(ky*kw+kx)*cin+ci, co]. */
+/* Weight gradient, TMA-fed (pixels = reduction dimension, both operands arrive as [pixel][channel] boxes = MN-major wgmma
+ * operands): dw_t (kh*kw*cin, cout) fp32 += the gradient (zeroed by the caller), dW[co,ci,ky,kx] = dw_t[(ky*kw+kx)*cin+ci, co]. */
 int esb_conv2d_tma_wgrad(const void* x, const void* dy, float* dw_t, int n_img, int H, int W, int cin, int cout, int kh,
                          int kw, int stride, int pad, void* stream);
 /* Input gradient (stride 1 or 2) with the same kernel: dx (n_img,H,W,cin) from dy (n_img,Ho,Wo,cout) and the forward filter as
@@ -159,7 +152,7 @@ int esb_conv3d_tma_dgrad(const void* dy, const void* w_odhwi, void* dx, int n, i
                          int stride, int pad, void* stream);
 int esb_conv3d_tma_wgrad(const void* x, const void* dy, float* dw_t, int n, int D, int H, int W, int cin, int cout, int k,
                          int stride, int pad, void* stream);
-/* The 7x7/2 stem on the 3-channel image as a tcgen05 implicit GEMM with the im2col rows built in shared memory
+/* The 7x7/2 stem on the 3-channel image as a wgmma implicit GEMM with the im2col rows built in shared memory
  * (csrc/conv_tma.cu::stem7x7_tc_kernel). x (n_img,H,W,3) bf16 NHWC, w_ohwi (16,7,7,3) bf16, bias (16) fp32, y (n_img,Ho,Wo,16). */
 int esb_stem7x7_tc(const void* x, const void* w_ohwi, const float* bias, void* y, int n_img, int H, int W, int relu,
                    void* stream);
@@ -180,9 +173,9 @@ int esb_maxpool2d_nhwc(const void* x, void* y, int n_img, int H, int W, int C, i
 
 /* ---- attention core of the grounding decoder (self-, text- and 3D cross-attention of
  * embodiedscan/models/layers/ground_transformer/decoder.py:89-95,151-177; †upstream nn.MultiheadAttention) as flash-attention
- * tiles on tcgen05 / TMEM fed by TMA (csrc/attn_tc.cu). Head dimension 32. q (B,H,Lq,32), k / v (B,H,Lk,32), o bf16 contiguous;
+ * tiles on wgmma fed by TMA (csrc/attn_tc.cu). Head dimension 32. q (B,H,Lq,32), k / v (B,H,Lk,32), o bf16 contiguous;
  * key_pad (B,Lk) uint8 (1 = ignore) or NULL; lse (B,H,Lq) fp32. Backward: delta (B,H,Lq) fp32 workspace, dq (B,H,Lq,32) fp32
- * ZEROED BY THE CALLER (key tiles accumulate with vector atomics), dk / dv (B,H,Lk,32) bf16 written once. -------------------- */
+ * += the gradient (zeroed by the caller; key tiles add in order), dk / dv (B,H,Lk,32) bf16 written once. ------------------- */
 int esb_attn_fwd(const void* q, const void* k, const void* v, const unsigned char* key_pad, void* o, float* lse, int B, int H,
                  int Lq, int Lk, float scale, void* stream);
 int esb_attn_bwd(const void* q, const void* k, const void* v, const unsigned char* key_pad, const void* o, const void* dout,

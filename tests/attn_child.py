@@ -1,4 +1,4 @@
-"""Child process: the tcgen05 flash-attention kernels (csrc/attn_tc.cu) against fp32 softmax attention on the bf16-rounded
+"""Child process: the wgmma flash-attention kernels (csrc/attn_tc.cu) against fp32 softmax attention on the bf16-rounded
 operands, forward and backward, with and without a key padding mask; one JSON line per case, `--bench` adds timings."""
 import json
 import os

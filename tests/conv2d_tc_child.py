@@ -1,4 +1,4 @@
-"""Child process of tests/test_a_golden_gpu.py::test_conv2d_tc_forward_matches_torch: runs the experimental tcgen05 conv2d
+"""Child process of tests/test_a_golden_gpu.py::test_conv2d_tc_forward_matches_torch: runs the experimental wgmma conv2d
 kernel against torch's fp32 convolution on bf16-rounded inputs and prints one JSON line per case."""
 import json
 import os

@@ -1,4 +1,4 @@
-"""Child process of tests/test_kernels_gpu.py::test_conv2d_tma_*: runs the TMA + tcgen05 conv2d kernel (csrc/conv_tma.cu)
+"""Child process of tests/test_kernels_gpu.py::test_conv2d_tma_*: runs the TMA + wgmma conv2d kernel (csrc/conv_tma.cu)
 against torch's fp32 convolution on bf16-rounded inputs, one JSON line per case (a first-run tensor-core kernel that hangs
 must not take the test session with it: the parent applies a timeout).  `--bench` adds C2-sized timings."""
 import json
@@ -27,7 +27,7 @@ CASES = [
 
 
 def run_stem(dev):
-    """The 7x7/2 stem (tcgen05 with shared-memory im2col) through the module-level dispatch of backbones._ConvBlock2D."""
+    """The 7x7/2 stem (wgmma with shared-memory im2col) through the module-level dispatch of backbones._ConvBlock2D."""
     from embodiedscan_b200.backbones import _ConvBlock2D
     for n, hw in ((2, (48, 64)), (3, (62, 90)), (1, (480, 640))):
         g = torch.Generator().manual_seed(n * 7 + hw[0])

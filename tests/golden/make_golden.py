@@ -604,7 +604,29 @@ def gen_metrics():
          occupancy_json=np.array(json.dumps({k: float(v) for k, v in ret_occ.items()}, sort_keys=True)))
 
 
-GENERATORS = dict(metrics=gen_metrics, continuous_occ=gen_continuous_occ, continuous=gen_continuous, augment=gen_augment, grounding=gen_grounding, detector=gen_detector, occupancy=gen_occupancy, frontend=gen_frontend, functions=gen_functions,
+def gen_model_configs():
+    """The `model = dict(...)` of the six reference config files the drop-in test builds (tests/test_reference_dropin_cpu.py),
+    stored as Python literals (repr) so that tuples survive."""
+    files = ['configs/detection/mv-det3d_8xb4_embodiedscan-3d-284class-9dof.py',
+             'configs/detection/cont-det3d_8xb1_embodiedscan-3d-284class-9dof.py',
+             'configs/occupancy/mv-occ_8xb1_embodiedscan-occ-80class.py',
+             'configs/occupancy/cont-occ_8xb1_embodiedscan-occ-80class.py',
+             'configs/grounding/mv-grounding_8xb12_embodiedscan-vg-9dof.py',
+             'configs/grounding/mv-grounding_8xb12_embodiedscan-vg-9dof_fcaf-coder.py']
+    import json
+
+    import embodiedscan
+    ref = os.path.dirname(os.path.abspath(list(embodiedscan.__path__)[0]))
+    out = {}
+    for f in files:
+        scope = {}
+        exec(compile(open(os.path.join(ref, f)).read(), f, 'exec'), scope)     # `_base_` files only hold runtime settings
+        out[f] = repr(scope['model'])
+    with open(os.path.join(HERE, 'reference_model_configs.json'), 'w') as fh:
+        json.dump(out, fh, indent=1)
+
+
+GENERATORS = dict(model_configs=gen_model_configs, metrics=gen_metrics, continuous_occ=gen_continuous_occ, continuous=gen_continuous, augment=gen_augment, grounding=gen_grounding, detector=gen_detector, occupancy=gen_occupancy, frontend=gen_frontend, functions=gen_functions,
                   eval=gen_eval)
 
 if __name__ == '__main__':

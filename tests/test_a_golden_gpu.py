@@ -8,13 +8,13 @@ Bar (BASELINE.json north_star): selection order / labels identical, fp32 values 
 Gradients of a 50-layer network with batch statistics over a few hundred rows are not that well conditioned: perturbing every
 weight of the fixture model by 1e-7 relative (about one fp32 ulp) moves the sampled gradients of `detector_g1` by 3e-5 of the
 tensor maximum on the CPU oracle — an amplification of ~300 — so two fp32 implementations that differ only in summation
-order (CPU BLAS vs fp32 atomics / tensor-core tiles) land 2e-3 .. 6e-3 apart (measured on the B200: 2.4e-3 and 5.5e-3 on the
-two tensors that tripped the former 2e-3 bound, the failing tensor changing from run to run and identical for the cuDNN and
-the library's own fp32 convolutions). The gradient bound is therefore 1e-2 of the tensor maximum for single entries and
+order (CPU BLAS vs fp32 atomics / tensor-core tiles) land 2e-3 .. 6e-3 apart (2.4e-3 and 5.5e-3 were seen on the two
+tensors that tripped the former 2e-3 bound, the failing tensor changing from run to run and identical for the cuDNN and the
+library's own fp32 convolutions). The gradient bound is therefore 1e-2 of the tensor maximum for single entries and
 5e-3 for the norm; the losses keep the 1e-3 bar.
 
-The file name sorts last on purpose: these tests were written after round 1's GPU budget was spent, so they run after
-the oracle-parity files that were green on the B200 (`-x` stops at the first failure)."""
+The file name sorts first: these tests compare the CUDA path with the stored outputs of the reference itself, ahead of the
+oracle-parity files (`-x` stops at the first failure)."""
 import pytest
 import torch
 
@@ -318,10 +318,9 @@ def test_detector_loss_is_invariant_to_the_row_order(monkeypatch):
 
 
 def test_conv2d_tc_forward_matches_torch():
-    """csrc/conv2d_tc.cu — the cp.async-gather tcgen05 conv2d family (forward, transposed-gather dgrad, split-K wgrad) that
-    csrc/conv_tma.cu superseded on the measured path; kept as the measured baseline of the TMA kernels (its first B200 run:
-    19 / 19 cases, profiles/r2_conv2d_tc_first_run.jsonl) and as the dgrad for strides above 2. Runs in a CHILD process with
-    a hard timeout like every first-run tensor-core kernel."""
+    """csrc/conv2d_tc.cu — the cp.async-gather wgmma conv2d family (forward, transposed-gather dgrad, split-K wgrad) that
+    csrc/conv_tma.cu superseded on the measured path; kept as the baseline of the TMA kernels and as the dgrad for strides
+    above 2. Runs in a CHILD process with a hard timeout like every first-run tensor-core kernel."""
     import json
     import os
     import subprocess

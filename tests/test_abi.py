@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, and exports exactly the symbols include/esb200.h declares
+"""CPU: the C-ABI library builds for sm_90a, loads, and exports exactly the symbols include/esb200.h declares
 (no compute calls without a GPU); the product path fails loudly without the library."""
 import ctypes
 import os

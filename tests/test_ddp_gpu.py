@@ -1,4 +1,4 @@
-"""2 x B200 over NCCL: the gradient arena after the bucketed, hook-launched all-reduce of a real detector step (2D side
+"""2 GPUs over NCCL: the gradient arena after the bucketed, hook-launched all-reduce of a real detector step (2D side
 stream overlap ON, direct-accumulation sparse-conv / BatchNorm gradients) equals the sum of the two ranks' single-rank
 gradients (SURVEY §4 (iv); engine.DataParallelReducer). Skipped on a one-GPU box."""
 import os

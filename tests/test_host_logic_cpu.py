@@ -1,5 +1,5 @@
 """Host-side logic of the product exercised without a GPU: the C-ABI call is replaced by a numpy emulation of the ONE
-kernel involved, so that batching / padding / bookkeeping code written while no B200 was available cannot hide a Python
+kernel involved, so that batching / padding / bookkeeping code cannot hide a Python
 error behind the GPU tests. The emulation lives only here; the product itself never falls back to the CPU."""
 import ctypes
 import os
@@ -190,8 +190,8 @@ def _emulate_conv2d_tc(src, wt, n_img, Hs, Ws, cs, Hr, Wr, cr, kh, kw, stride, p
 
 
 def test_conv2d_tc_index_arithmetic_forward_and_transposed():
-    """The gather formulas and the weight packings of the experimental tcgen05 conv2d (forward and dgrad mode) reproduce
-    F.conv2d and its input gradient when evaluated literally on the CPU (the tensor-core plumbing itself needs a B200)."""
+    """The gather formulas and the weight packings of the experimental wgmma conv2d (forward and dgrad mode) reproduce
+    F.conv2d and its input gradient when evaluated literally on the CPU (the tensor-core plumbing itself needs an H100)."""
     import torch.nn.functional as F
     from embodiedscan_b200.backbones import pack_ohwi
     g = torch.Generator().manual_seed(0)

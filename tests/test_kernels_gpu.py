@@ -137,7 +137,7 @@ def test_spconv_fwd_bwd(cin, cout, ksize, stride, dtype):
     y = conv(SP.SparseTensor(xd, coordinate_map_key=key, coordinate_manager=mgr))
     assert np.array_equal(y.C.cpu().numpy().astype(np.int64), out_c)
     y.F.backward(gy.to(_dev(), dtype))
-    # bf16 storage (8-bit mantissa outputs); the tcgen05 path (channels % 64 == 0) accumulates in fp32 TMEM
+    # bf16 storage (8-bit mantissa outputs); the wgmma path (channels % 64 == 0) accumulates in fp32 registers
     tol = RTOL if dtype == torch.float32 else 2e-2
     _close(y.F, yr, tol, 'fwd')
     _close(xd.grad, xr.grad, tol, 'dgrad')
@@ -546,7 +546,7 @@ def _run_child(script, *args, timeout=420):
 
 
 def test_conv2d_tma_family_matches_torch():
-    """csrc/conv_tma.cu: TMA + tcgen05 conv2d forward (stride 1 / 2, 32B / 64B / 128B swizzle, fused epilogue), stride-1 and
+    """csrc/conv_tma.cu: TMA + wgmma conv2d forward (stride 1 / 2, 32B / 64B / 128B swizzle, fused epilogue), stride-1 and
     stride-2 dgrad (filter read MN-major, parity-class stores), TMA-fed wgrad and the shared-memory-im2col stem, against torch
     fp32 on bf16-rounded operands (1e-2 of the tensor maximum: bf16 output rounding)."""
     rows = _run_child('conv_tma_child.py')
@@ -554,14 +554,6 @@ def test_conv2d_tma_family_matches_torch():
     assert not bad, bad
     kinds = {r['kind'] for r in rows}
     assert {'fwd', 'dgrad', 'wgrad', 'stem', 'conv3d'} <= kinds, kinds
-
-
-def test_spconv_tma_matches_cp_async_kernels():
-    """csrc/spconv_tma.cu (gather4 rows, tiled filter boxes, M = 256 tiles) vs csrc/spconv_tc.cu on the same maps."""
-    rows = _run_child('spconv_tma_child.py')
-    bad = [r for r in rows if not r.get('ok', True)]
-    assert not bad, bad
-    assert sum(r['kind'] == 'parity' for r in rows) >= 9
 
 
 def test_union_add_and_interp_kernels():
@@ -645,7 +637,7 @@ def test_fused_batchnorm_bf16_matches_reference():
 
 
 def test_flash_attention_tc_matches_softmax_attention():
-    """csrc/attn_tc.cu (tcgen05 flash attention, forward + dq / dk / dv) against fp32 softmax attention on bf16-rounded
+    """csrc/attn_tc.cu (wgmma flash attention, forward + dq / dk / dv) against fp32 softmax attention on bf16-rounded
     operands: self-attention, padded keys, 3.5k keys, ragged sizes below one tile."""
     rows = _run_child('attn_child.py')
     bad = [r for r in rows if not r.get('ok', True)]

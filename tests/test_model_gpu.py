@@ -314,7 +314,7 @@ def test_grounder_predict_matches_oracle():
 def test_c2_shaped_bf16_step_matches_oracle():
     """Parity AT THE HEADLINE SHAPE: one C2 scan (20 views 480x640, 100k points, ResNet-50/16 + MinkResNet34) against the fp32
     CPU oracle on the same weights and inputs, through (a) the fp32 parity arithmetic of the CUDA path and (b) the bf16
-    throughput path (tcgen05 / TMA kernels, CUDA-graphed 2D branch, fused BatchNorm).
+    throughput path (wgmma / TMA kernels, CUDA-graphed 2D branch, fused BatchNorm).
     Losses: (a) 1e-3, (b) 2e-3 relative (measured 1e-4). Gradients: (a) must match the oracle in direction and size on every
     watched tensor; (b) must match on the head's classifier, whose gradient is well conditioned — deeper tensors are reported
     only: with batch statistics over one scan a round-off perturbation of the weights is amplified ~x300 on its way into the

@@ -1,21 +1,25 @@
-"""Drop-in check against the reference tree itself (dev container only: skipped where /root/reference is absent, e.g. on
-the GPU box). With the third-party stand-ins of tests/golden/refstubs.py installed, `register_into_reference()` must make
-the reference's OWN registry build the esb200 classes from the reference's UNMODIFIED config files."""
+"""Drop-in check against the reference's registry: `register_into_reference()` must make the registry the reference's
+tools build from (`embodiedscan.registry.MODELS`) produce the esb200 classes from the reference's UNMODIFIED model configs.
+The `model = dict(...)` of each config file is stored in tests/golden/reference_model_configs.json (Python literals,
+written by `tests/golden/make_golden.py model_configs`); the registry is the mmengine stand-in of tests/golden/refstubs.py,
+installed as `embodiedscan.registry` for the duration of the test. Like the reference, which registers its own classes
+under these names first, the stand-in starts with a placeholder under every name; building one means
+`register_into_reference()` did not override it."""
+import ast
+import json
 import os
 import sys
+import types
 
 import pytest
 
-REF = '/root/reference'
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, 'embodiedscan')), reason='needs /root/reference')
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
+CONFIGS = json.load(open(os.path.join(GOLD, 'reference_model_configs.json')))
 
 
-def load_config(path):
-    """The `model = dict(...)` of an mmengine python config (plain exec; `_base_` files only hold runtime settings)."""
-    scope = {}
-    exec(compile(open(path).read(), path, 'exec'), scope)
-    return scope['model']
+def load_config(cfg_file):
+    """The stored `model = dict(...)` of a reference config file."""
+    return ast.literal_eval(CONFIGS[cfg_file])
 
 
 @pytest.mark.parametrize('cfg_file,cls_name', [
@@ -26,23 +30,35 @@ def load_config(path):
     ('configs/grounding/mv-grounding_8xb12_embodiedscan-vg-9dof.py', 'SparseFeatureFusion3DGrounder'),
     ('configs/grounding/mv-grounding_8xb12_embodiedscan-vg-9dof_fcaf-coder.py', 'SparseFeatureFusion3DGrounder'),
 ])
-def test_reference_registry_builds_esb200_from_unmodified_configs(cfg_file, cls_name):
+def test_reference_registry_builds_esb200_from_unmodified_configs(cfg_file, cls_name, monkeypatch):
     if GOLD not in sys.path:
         sys.path.insert(0, GOLD)
     import refstubs
-    refstubs.install(REF)
-    import embodiedscan.models  # noqa: F401  (the reference registers its own classes first)
-    from embodiedscan.registry import MODELS as REF_MODELS
+    pkg = types.ModuleType('embodiedscan')
+    reg = types.ModuleType('embodiedscan.registry')
+    reg.MODELS, reg.TASK_UTILS = refstubs.Registry('model'), refstubs.Registry('task util')
+    pkg.registry = reg
+    monkeypatch.setitem(sys.modules, 'embodiedscan', pkg)
+    monkeypatch.setitem(sys.modules, 'embodiedscan.registry', reg)
 
     import embodiedscan_b200
-    from embodiedscan_b200.registry import register_into_reference
+    from embodiedscan_b200.registry import MODELS, TASK_UTILS, register_into_reference
+
+    def placeholder(name):
+        def init(self, *args, **kwargs):
+            raise AssertionError(f'the reference class {name} was built: register_into_reference() did not override it')
+        return type(name, (), {'__init__': init})
+
+    for ours, theirs in ((MODELS, reg.MODELS), (TASK_UTILS, reg.TASK_UTILS)):
+        for name in ours._module_dict:
+            theirs.register_module(name=name, module=placeholder(name))
     register_into_reference()
-    model_cfg = load_config(os.path.join(REF, cfg_file))
+    model_cfg = load_config(cfg_file)
     assert model_cfg['type'] == cls_name
     for sub in ('backbone', 'neck'):                      # pretrained-checkpoint URLs need a network
         if isinstance(model_cfg.get(sub), dict):
             model_cfg[sub].pop('init_cfg', None)
-    model = REF_MODELS.build(model_cfg)
+    model = reg.MODELS.build(model_cfg)
     assert type(model).__module__.startswith('embodiedscan_b200'), type(model)
     assert type(model) is getattr(embodiedscan_b200, cls_name, None) or type(model).__name__ == cls_name
     names = dict(model.named_parameters())
