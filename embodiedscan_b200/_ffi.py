@@ -44,9 +44,6 @@ SIGNATURES = {
     'esb_gather2_rows': ('ppqpppqiip', 'i'),
     'esb_head_split_fwd': ('pppqiiiifppppp', 'i'),
     'esb_head_split_bwd': ('pppppqiiiifpppp', 'i'),
-    'esb_conv2d_tc_fwd': ('ppppp' + 'iiiiiiiiiii' + 'p', 'i'),
-    'esb_conv2d_tc_dgrad': ('ppp' + 'iiiiiiiiii' + 'p', 'i'),
-    'esb_conv2d_tc_wgrad': ('ppp' + 'iiiiiiiii' + 'p', 'i'),
     'esb_conv2d_tma_fwd': ('ppppp' + 'iiiiiiiiii' + 'p', 'i'),
     'esb_conv2d_tma_wgrad': ('ppp' + 'iiiiiiiii' + 'p', 'i'),
     'esb_conv2d_tma_dgrad': ('ppp' + 'iiiiiiiii' + 'p', 'i'),

@@ -121,27 +121,6 @@ class _BiasResAct(torch.autograd.Function):
         return g, None, (g if ctx.has_res else None), None
 
 
-def conv2d_tc(x: torch.Tensor, w_ohwi: torch.Tensor, bias, res, relu: bool, kh: int, kw: int, stride: int, pad: int):
-    """The folded conv + bias + residual + ReLU block in ONE wgmma implicit-GEMM launch with a cp.async gather
-    (csrc/conv2d_tc.cu: the measured baseline of csrc/conv_tma.cu). x (N,Cin,H,W) bf16 in channels_last memory; w_ohwi (Cout, r_pad) bf16 from
-    :func:`pack_ohwi`; bias (Cout,) fp32 or None; res like the output or None. Forward only (frozen / inference)."""
-    from . import _ffi
-    assert x.is_cuda and x.dtype == torch.bfloat16 and x.is_contiguous(memory_format=torch.channels_last)
-    N, cin, H, W = x.shape
-    cout, r_pad = w_ohwi.shape
-    Ho, Wo = (H + 2 * pad - kh) // stride + 1, (W + 2 * pad - kw) // stride + 1
-    y = torch.empty((N, cout, Ho, Wo), dtype=torch.bfloat16, device=x.device, memory_format=torch.channels_last)
-    if res is not None:
-        assert res.shape == y.shape and res.dtype == torch.bfloat16
-        if not res.is_contiguous(memory_format=torch.channels_last):
-            res = res.contiguous(memory_format=torch.channels_last)
-    if bias is not None:
-        bias = bias.float().contiguous()
-    _ffi.call('esb_conv2d_tc_fwd', x.data_ptr(), w_ohwi.data_ptr(), _ffi.ptr(bias), _ffi.ptr(res), y.data_ptr(), N, H, W,
-              cin, cout, kh, kw, stride, pad, r_pad, 1 if relu else 0, _ffi.stream())
-    return y
-
-
 def ohwi(w: torch.Tensor) -> torch.Tensor:
     """(Cout, Cin, kh, kw) -> contiguous (Cout, kh, kw, Cin) bf16: the filter matrix of csrc/conv_tma.cu (a channels_last
     filter already is this memory: no copy then)."""
@@ -198,53 +177,10 @@ def conv2d_tma_dgrad(dy: torch.Tensor, w_ohwi: torch.Tensor, in_hw, pad: int, st
     return dx
 
 
-def pack_ohwi(w: torch.Tensor) -> torch.Tensor:
-    """(Cout, Cin, kh, kw) -> (Cout, r_pad) bf16: filter taps in (ky, kx, ci) order, rows zero padded to a multiple of
-    64 reduction elements — the K-major B operand of csrc/conv2d_tc.cu."""
-    cout = w.shape[0]
-    flat = w.detach().permute(0, 2, 3, 1).reshape(cout, -1)
-    r = flat.shape[1]
-    r_pad = (r + 63) // 64 * 64
-    out = torch.zeros((cout, r_pad), dtype=torch.bfloat16, device=w.device)
-    out[:, :r] = flat.to(torch.bfloat16)
-    return out
-
-
-def conv2d_tc_dgrad(dy: torch.Tensor, w: torch.Tensor, in_hw, stride: int, pad: int) -> torch.Tensor:
-    """dL/dx of ``F.conv2d(x, w, stride, pad)`` with the same kernel in transposed-gather mode.
-    dy (N,Cout,Ho,Wo) bf16 channels_last; w (Cout,Cin,kh,kw); returns dx (N,Cin,H,W) bf16 channels_last."""
-    from . import _ffi
-    assert dy.is_cuda and dy.dtype == torch.bfloat16 and dy.is_contiguous(memory_format=torch.channels_last)
-    cout, cin, kh, kw = w.shape
-    H, W = in_hw
-    flat = w.detach().permute(1, 2, 3, 0).reshape(cin, -1)             # (ci | ky, kx, co)
-    r = flat.shape[1]
-    r_pad = (r + 63) // 64 * 64
-    wt = torch.zeros((cin, r_pad), dtype=torch.bfloat16, device=w.device)
-    wt[:, :r] = flat.to(torch.bfloat16)
-    dx = torch.empty((dy.shape[0], cin, H, W), dtype=torch.bfloat16, device=dy.device, memory_format=torch.channels_last)
-    _ffi.call('esb_conv2d_tc_dgrad', dy.data_ptr(), wt.data_ptr(), dx.data_ptr(), dy.shape[0], H, W, cin, cout, kh, kw,
-              stride, pad, r_pad, _ffi.stream())
-    return dx
-
-
-def conv2d_tc_wgrad(x: torch.Tensor, dy: torch.Tensor, w_shape, stride: int, pad: int) -> torch.Tensor:
-    """dL/dw of ``F.conv2d(x, w, stride, pad)``; x (N,Cin,H,W), dy (N,Cout,Ho,Wo) bf16 channels_last ->
-    (Cout,Cin,kh,kw) fp32 (split-K partial sums are added in a fixed order: the same bits on every run)."""
-    from . import _ffi
-    cout, cin, kh, kw = w_shape
-    assert x.dtype == dy.dtype == torch.bfloat16 and x.is_contiguous(memory_format=torch.channels_last) \
-        and dy.is_contiguous(memory_format=torch.channels_last)
-    dw_t = torch.zeros((kh * kw * cin, cout), dtype=torch.float32, device=x.device)
-    _ffi.call('esb_conv2d_tc_wgrad', x.data_ptr(), dy.data_ptr(), dw_t.data_ptr(), x.shape[0], x.shape[2], x.shape[3], cin,
-              cout, kh, kw, stride, pad, _ffi.stream())
-    return dw_t.view(kh, kw, cin, cout).permute(3, 2, 0, 1)
-
-
 class _ConvBlock2D(torch.autograd.Function):
     """out = act(conv2d(x, w) + bias + res) of the image backbone on the library's own kernels, all three passes:
-      bf16, tensor-core channel counts -> csrc/conv_tma.cu (TMA + wgmma; fused epilogue), its stride-1 dgrad, the
-                                         transposed-gather dgrad of csrc/conv2d_tc.cu for stride 2, wgmma split-K wgrad
+      bf16, tensor-core channel counts -> csrc/conv_tma.cu (TMA + wgmma; fused epilogue), its stride-1 / stride-2 dgrad
+                                         and its wgrad; the dgrad of larger strides -> csrc/conv2d_direct.cu
       fp32 (the parity arithmetic) / the 3-channel stem -> csrc/conv2d_direct.cu (fp32 FMA)
     x channels_last; w (Cout,Cin,kh,kw) in channels_last memory (= OHWI); bias fp32 (Cout,) constant; res like the output."""
 
@@ -297,8 +233,6 @@ class _ConvBlock2D(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             if tma and stride in (1, 2):
                 dx = conv2d_tma_dgrad(g, w_ohwi, (H, W), pad, stride)
-            elif tma:
-                dx = conv2d_tc_dgrad(g, w_ohwi.permute(0, 3, 1, 2), (H, W), stride, pad)
             else:
                 dx = torch.empty_like(x)
                 _ffi.call('esb_conv2d_direct_dgrad', g.data_ptr(), w_ohwi.data_ptr(), dx.data_ptr(), N, H, W, cin, cout, kh,
@@ -327,13 +261,6 @@ def maxpool2d(x: torch.Tensor, k: int, stride: int, pad: int) -> torch.Tensor:
                   _ffi.stream())
         return y
     return F.max_pool2d(x, kernel_size=k, stride=stride, padding=pad)
-
-
-def conv2d_backend() -> str:
-    """'own' (default: every 2D convolution on the library's kernels, see :class:`_ConvBlock2D`) or 'cudnn'
-    (ESB200_CONV2D=cudnn: the round-1 library path, kept for A/B timing only)."""
-    import os
-    return os.environ.get('ESB200_CONV2D', 'own')
 
 
 class _ConvBN(nn.Module):
@@ -381,7 +308,7 @@ class _ConvBN(nn.Module):
             w = self._const_w.get(x.dtype)
             if w is None:
                 w = self._const_w[x.dtype] = (conv.weight.detach() * scale4).to(x.dtype)
-        if (conv2d_backend() == 'own' and x.is_cuda and x.dtype in (torch.float32, torch.bfloat16) and not b.requires_grad
+        if (x.is_cuda and x.dtype in (torch.float32, torch.bfloat16) and not b.requires_grad
                 and conv.stride[0] == conv.stride[1] and conv.padding[0] == conv.padding[1]):
             # the library's own kernels, all three passes (conv + bias + residual + ReLU fused into one launch)
             if not x.is_contiguous(memory_format=torch.channels_last):
@@ -542,7 +469,7 @@ class ResNet(nn.Module):
         import os
         c = self._graph_lists()
         return (x.is_cuda and self.training and torch.is_grad_enabled() and x.dtype == torch.bfloat16
-                and conv2d_backend() == 'own' and os.environ.get('ESB200_GRAPH2D', '1') != '0'
+                and os.environ.get('ESB200_GRAPH2D', '1') != '0'
                 and not torch.cuda.is_current_stream_capturing()
                 and all(not b.training for b in c['bns']) and any(p.requires_grad for p in c['params']))
 

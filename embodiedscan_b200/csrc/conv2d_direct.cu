@@ -1,8 +1,10 @@
 // esb200 — direct (SIMT, fp32-accumulate) NHWC 2D convolution, its two gradients and the stem's max pooling.
-// Two jobs on the per-view image backbone (SURVEY §8 row a5; mmdet.ResNet called at
+// Three jobs on the per-view image backbone (SURVEY §8 row a5; mmdet.ResNet called at
 // embodiedscan/models/detectors/sparse_featfusion_single_stage.py:130-136):
-//   * the fp32 PARITY arithmetic of every 2D convolution (the wgmma kernels of conv_tma.cu / conv2d_tc.cu take bf16
-//     operands; fp32 FMA is what the 1e-3 bound of BASELINE.json is checked in), forward, dgrad and wgrad;
+//   * the fp32 PARITY arithmetic of every 2D convolution (the wgmma kernels of conv_tma.cu take bf16 operands; fp32 FMA
+//     is what the 1e-3 bound of BASELINE.json is checked in), forward, dgrad and wgrad;
+//   * the bf16 dgrad of a TMA-sized convolution with stride > 2, which conv_tma.cu's dgrad does not take (one thread per
+//     input pixel: no atomics, so the result stays deterministic);
 //   * the 7x7/2 stem on the 3-channel image in either dtype (Cin = 3 cannot feed a 16-byte TMA box) and the 3x3/2 max pool.
 // Layouts: x (n,H,W,cin), w OHWI (cout,kh,kw,cin), y (n,Ho,Wo,cout); T = float or bf16, accumulation fp32.
 // Roofline: fp32 FMA for the stem (147 x 16 FMA per output pixel), HBM for the pool.

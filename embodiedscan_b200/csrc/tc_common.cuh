@@ -1,5 +1,5 @@
 // esb200 — wgmma / mbarrier / cp.async / TMA primitives shared by every tensor-core kernel of the library
-// (spconv_tc.cu, conv2d_tc.cu, conv_tma.cu, attn_tc.cu): ONE copy of the descriptor encoders.
+// (spconv_tc.cu, conv_tma.cu, attn_tc.cu): ONE copy of the descriptor encoders.
 #pragma once
 #include <cuda.h>            // CUtensorMap (types only: the encoder is fetched through cudaGetDriverEntryPoint)
 #include "common.cuh"
@@ -56,11 +56,6 @@ __device__ __forceinline__ void acc_fence(float* d) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-template <int R>
-__device__ __forceinline__ void acc_zero(float* d) {
-#pragma unroll
-  for (int i = 0; i < R; ++i) d[i] = 0.f;
-}
 // m64nN fp32 fragment layout: element i of thread t (0..127 in the warpgroup) is row 16*(t/32) + (t%32)/4 + 8*((i/2)%2),
 // column 8*(i/4) + 2*(t%4) + i%2.
 template <int N>
@@ -110,26 +105,10 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(dst), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tma_load_3d(const CUtensorMap* m, uint64_t* bar, uint32_t dst, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-               ::"r"(dst), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar, uint32_t dst, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(dst), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
 __device__ __forceinline__ void tma_load_5d(const CUtensorMap* m, uint64_t* bar, uint32_t dst, int c0, int c1, int c2, int c3,
                                             int c4) {
   asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
                ::"r"(dst), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(m), "r"(src), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"(m), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 __device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3, int c4) {
   asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"

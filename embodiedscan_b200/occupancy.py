@@ -85,8 +85,7 @@ def _tma3d_ok(x, conv) -> bool:
     """The dense 3-D stack runs on the library's TMA + wgmma kernels (csrc/conv_tma.cu, rank-5 tensor maps) when the
     activations are bf16 on the GPU and the channel counts tile (16, 32, multiples of 64; outputs a power of two <= 256 or a
     multiple of 256); anything else (fp32 parity arithmetic, toy widths) stays on the library convolution."""
-    import os
-    if not (x.is_cuda and x.dtype == torch.bfloat16 and os.environ.get('ESB200_CONV3D', 'own') == 'own'):
+    if not (x.is_cuda and x.dtype == torch.bfloat16):
         return False
     cin, cout = (conv.in_channels, conv.out_channels)
 

@@ -109,23 +109,6 @@ int esb_act_bwd(const void* dy, const void* y, void* dx, long long n, int act, i
  * row gathers of its backward. C % 8 == 0. */
 int esb_gather2_rows(const void* a, const int* ia, long long na, const void* b, const int* ib, void* out, long long n, int C,
                      int dtype, void* stream);
-/* cp.async-gather baseline of the TMA kernels below (csrc/conv2d_tc.cu): the folded conv+BN(+residual)(+ReLU) block of the per-view 2D
- * ResNet (mmdet.ResNet called at embodiedscan/models/detectors/sparse_featfusion_single_stage.py:130-136) as ONE
- * wgmma implicit GEMM. x (n_img,H,W,cin) bf16 NHWC; w_ohwi (cout, r_pad) bf16 = the filter in (ky,kx,ci) order,
- * each row zero padded from kh*kw*cin to r_pad (multiple of 64); bias (cout) fp32 or NULL; residual / y
- * (n_img,Ho,Wo,cout) bf16 NHWC, residual may be NULL. cin % 8 == 0, cout % 8 == 0. */
-int esb_conv2d_tc_fwd(const void* x, const void* w_ohwi, const float* bias, const void* residual, void* y, int n_img,
-                      int H, int W, int cin, int cout, int kh, int kw, int stride, int pad, int r_pad, int relu,
-                      void* stream);
-/* Input gradient of the same convolution (transposed-gather mode of the same kernel). dy
- * (n_img,Ho,Wo,cout) bf16 NHWC; w_ihwo (cin, r_pad) bf16 = the filter as (ci | ky,kx,co), rows zero padded from
- * kh*kw*cout to r_pad; dx (n_img,H,W,cin) bf16 NHWC, every element written once. */
-int esb_conv2d_tc_dgrad(const void* dy, const void* w_ihwo, void* dx, int n_img, int H, int W, int cin, int cout,
-                        int kh, int kw, int stride, int pad, int r_pad, void* stream);
-/* Weight gradient (pixels are the reduction dimension, split over CTAs). dw_t (kh*kw*cin, cout) fp32,
- * zeroed by the caller, row r = (ky,kx,ci): dW[co,ci,ky,kx] = dw_t[(ky*kw+kx)*cin+ci, co]. */
-int esb_conv2d_tc_wgrad(const void* x, const void* dy, float* dw_t, int n_img, int H, int W, int cin, int cout, int kh,
-                        int kw, int stride, int pad, void* stream);
 /* The per-view 2D backbone's convolution as a persistent TMA + wgmma implicit GEMM (csrc/conv_tma.cu): activations,
  * filter and output move with cp.async.bulk.tensor tiles (zero padding = TMA out-of-bounds fill, stride = tensor-map element
  * strides), accumulators live in registers, bias + residual + ReLU are fused into the epilogue. Replaces the cuDNN call behind

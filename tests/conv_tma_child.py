@@ -93,6 +93,36 @@ def run_conv3d(dev):
         print(json.dumps(res), flush=True)
 
 
+def run_dispatch(dev):
+    """A bf16 convolution with TMA-sized channels and stride 3 through backbones._ConvBlock2D, forward and backward: the
+    TMA forward and wgrad, and the dgrad of csrc/conv2d_direct.cu (the TMA dgrad takes strides 1 and 2 only), against
+    torch fp32 on bf16-rounded operands."""
+    from embodiedscan_b200.backbones import _ConvBlock2D
+    cin, cout, k, stride, pad, hw, n = 64, 64, 3, 3, 1, (31, 41), 2
+    g = torch.Generator().manual_seed(3)
+    x = torch.randn(n, cin, *hw, generator=g).bfloat16()
+    w = (torch.randn(cout, cin, k, k, generator=g) / (cin * k * k) ** 0.5).bfloat16()
+    b = torch.randn(cout, generator=g)
+    xr, wr = x.float().requires_grad_(True), w.float().requires_grad_(True)
+    ref = F.conv2d(xr, wr, b, stride, pad)
+    dy = torch.randn(ref.shape, generator=g).bfloat16()
+    ref.backward(dy.float())
+    xd = x.to(dev).contiguous(memory_format=torch.channels_last).requires_grad_(True)
+    wd = w.to(dev).contiguous(memory_format=torch.channels_last).requires_grad_(True)
+    out = _ConvBlock2D.apply(xd, wd, b.to(dev), None, False, stride, pad)
+    out.backward(dy.to(dev).contiguous(memory_format=torch.channels_last))
+    torch.cuda.synchronize()
+    res = dict(kind='dispatch', case=[cin, cout, k, stride, pad, list(hw), n])
+    ok = tuple(out.shape) == tuple(ref.shape)
+    for name, a, r in (('fwd', out, ref), ('dgrad', xd.grad, xr.grad), ('wgrad', wd.grad, wr.grad)):
+        err = float((a.float().cpu() - r.detach()).abs().max())
+        tol = 1e-2 * max(float(r.detach().abs().max()), 1.0)
+        res[name] = err
+        ok = ok and err <= tol
+    res['ok'] = bool(ok)
+    print(json.dumps(res), flush=True)
+
+
 def run_case(case, dev):
     from embodiedscan_b200.backbones import conv2d_tma, conv2d_tma_dgrad, ohwi
     cin, cout, k, stride, pad, hw, n, with_res = case
@@ -170,23 +200,20 @@ def bench(dev, n=80):
             torch.cuda.synchronize()
             ms[name] = e0.elapsed_time(e1) / 10
         byt = (x.numel() + y.numel() + w.numel()) * 2
-        from embodiedscan_b200.backbones import conv2d_tc_wgrad, conv2d_tma_wgrad
+        from embodiedscan_b200.backbones import conv2d_tma_wgrad
         dyb = torch.randn_like(y)
-        for name, fn in (('wgrad_tma', lambda: conv2d_tma_wgrad(x, dyb, tuple(w.shape), stride, pad)),
-                         ('wgrad_tc', lambda: conv2d_tc_wgrad(x, dyb, tuple(w.shape), stride, pad))):
-            for _ in range(2):
-                fn()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(5):
-                fn()
-            e1.record()
-            torch.cuda.synchronize()
-            ms[name] = e0.elapsed_time(e1) / 5
+        for _ in range(2):
+            conv2d_tma_wgrad(x, dyb, tuple(w.shape), stride, pad)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(5):
+            conv2d_tma_wgrad(x, dyb, tuple(w.shape), stride, pad)
+        e1.record()
+        torch.cuda.synchronize()
+        ms['wgrad_tma'] = e0.elapsed_time(e1) / 5
         print(json.dumps(dict(kind='bench', case=[cin, cout, k, stride, pad, list(hw), n], us_tma=1e3 * ms['tma'],
                               us_cudnn=1e3 * ms['cudnn'], gbs_tma=byt / ms['tma'] / 1e6, mbytes=byt / 1e6,
-                              us_wgrad_tma=1e3 * ms['wgrad_tma'], us_wgrad_tc=1e3 * ms['wgrad_tc'],
-                              gbs_wgrad_tma=byt / ms['wgrad_tma'] / 1e6)), flush=True)
+                              us_wgrad_tma=1e3 * ms['wgrad_tma'], gbs_wgrad_tma=byt / ms['wgrad_tma'] / 1e6)), flush=True)
 
 
 def main():
@@ -204,6 +231,10 @@ def main():
     except Exception as e:  # noqa
         print(json.dumps(dict(kind='error', case='stem', ok=False, err=str(e)[:300])), flush=True)
     if not only:
+        try:
+            run_dispatch(dev)
+        except Exception as e:  # noqa
+            print(json.dumps(dict(kind='error', case='dispatch', ok=False, err=str(e)[:300])), flush=True)
         try:
             run_conv3d(dev)
         except Exception as e:  # noqa

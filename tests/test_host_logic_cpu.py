@@ -161,75 +161,6 @@ def test_morton_row_order_is_stable_and_hierarchical():
         assert bool((k[1:] > k[:-1]).all()), f'stride-{stride} parents inherit the order'
 
 
-def _emulate_conv2d_tc(src, wt, n_img, Hs, Ws, cs, Hr, Wr, cr, kh, kw, stride, pad, r_pad, transposed):
-    """Index arithmetic of csrc/conv2d_tc.cu's producer, spelled out per (row pixel, 16-byte piece) in numpy:
-    src (n_img,Hs,Ws,cs) NHWC, wt (cr, r_pad) K-major weights -> (n_img*Hr*Wr, cr). Mirrors the kernel's formulas
-    line by line (iy0/ix0, tap/ch split of the reduction index, exact-division test of the transposed mode)."""
-    M = n_img * Hr * Wr
-    A = np.zeros((M, r_pad), np.float32)
-    taps = kh * kw
-    for m in range(M):
-        n, rem = divmod(m, Hr * Wr)
-        oy, ox = divmod(rem, Wr)
-        iy0 = oy + pad if transposed else oy * stride - pad
-        ix0 = ox + pad if transposed else ox * stride - pad
-        for r0 in range(0, r_pad, 8):
-            tap, ch = divmod(r0, cs)
-            ky, kx = divmod(tap, kw)
-            ok = tap < taps
-            if not transposed:
-                iy, ix = iy0 + ky, ix0 + kx
-            else:
-                ny, nx = iy0 - ky, ix0 - kx
-                iy, ix = int(ny / stride), int(nx / stride)          # C division truncates toward zero
-                ok = ok and ny >= 0 and nx >= 0 and iy * stride == ny and ix * stride == nx
-            ok = ok and 0 <= iy < Hs and 0 <= ix < Ws
-            if ok:
-                A[m, r0:r0 + 8] = src[n, iy, ix, ch:ch + 8]
-    return A @ wt.T
-
-
-def test_conv2d_tc_index_arithmetic_forward_and_transposed():
-    """The gather formulas and the weight packings of the experimental wgmma conv2d (forward and dgrad mode) reproduce
-    F.conv2d and its input gradient when evaluated literally on the CPU (the tensor-core plumbing itself needs an H100)."""
-    import torch.nn.functional as F
-    from embodiedscan_b200.backbones import pack_ohwi
-    g = torch.Generator().manual_seed(0)
-    for cin, cout, k, stride, pad, hw in ((16, 8, 3, 1, 1, (6, 7)), (8, 16, 3, 2, 1, (7, 9)), (16, 24, 1, 2, 0, (6, 8)),
-                                          (8, 8, 7, 2, 3, (12, 10))):
-        n = 2
-        x = torch.randn(n, cin, *hw, generator=g).bfloat16().float()
-        w = torch.randn(cout, cin, k, k, generator=g).bfloat16().float()
-        H, W = hw
-        Ho, Wo = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
-        xr = x.clone().requires_grad_(True)
-        ref = F.conv2d(xr, w, None, stride, pad)
-        wp = pack_ohwi(w).float().numpy()
-        out = _emulate_conv2d_tc(x.permute(0, 2, 3, 1).numpy(), wp, n, H, W, cin, Ho, Wo, cout, k, k, stride, pad,
-                                 wp.shape[1], False)
-        want = ref.detach().permute(0, 2, 3, 1).reshape(-1, cout).numpy()
-        assert np.abs(out - want).max() <= 1e-3 * max(np.abs(want).max(), 1), (cin, cout, k, stride)
-        dy = torch.randn(ref.shape, generator=g).bfloat16().float()
-        ref.backward(dy)
-        flat = w.permute(1, 2, 3, 0).reshape(cin, -1)                    # (ci | ky, kx, co), as conv2d_tc_dgrad packs it
-        r_pad = (flat.shape[1] + 63) // 64 * 64
-        wt = np.zeros((cin, r_pad), np.float32)
-        wt[:, :flat.shape[1]] = flat.numpy()
-        dx = _emulate_conv2d_tc(dy.permute(0, 2, 3, 1).numpy(), wt, n, Ho, Wo, cout, H, W, cin, k, k, stride, pad, r_pad,
-                                True)
-        want = xr.grad.permute(0, 2, 3, 1).reshape(-1, cin).numpy()
-        assert np.abs(dx - want).max() <= 1e-3 * max(np.abs(want).max(), 1), ('dgrad', cin, cout, k, stride)
-        # wgrad: dW^T[r, co] = sum_m A[m, r] dy[m, co] with the forward's implicit A, unpacked like conv2d_tc_wgrad
-        wr = w.clone().requires_grad_(True)
-        F.conv2d(x, wr, None, stride, pad).backward(dy)
-        eye = np.eye(wp.shape[1], dtype=np.float32)                       # identity weights expose A itself
-        A = _emulate_conv2d_tc(x.permute(0, 2, 3, 1).numpy(), eye, n, H, W, cin, Ho, Wo, wp.shape[1], k, k, stride, pad,
-                               wp.shape[1], False)
-        dw_t = A.T @ dy.permute(0, 2, 3, 1).reshape(-1, cout).numpy()
-        dw = torch.from_numpy(dw_t[:k * k * cin]).view(k, k, cin, cout).permute(3, 2, 0, 1)
-        assert float((dw - wr.grad).abs().max()) <= 1e-3 * max(float(wr.grad.abs().max()), 1), ('wgrad', cin, cout, k)
-
-
 def test_continuous_occupancy_view_prefix_painting_control_flow(monkeypatch):
     """EmbodiedOccPredictor.extract_feat with the CUDA pieces replaced by recorders: prefix idx paints the whole prior
     grid from feat2d[:idx+1] with its own projection prefix; volumes are stacked per prefix and fused with the sparse

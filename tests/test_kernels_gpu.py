@@ -547,13 +547,14 @@ def _run_child(script, *args, timeout=420):
 
 def test_conv2d_tma_family_matches_torch():
     """csrc/conv_tma.cu: TMA + wgmma conv2d forward (stride 1 / 2, 32B / 64B / 128B swizzle, fused epilogue), stride-1 and
-    stride-2 dgrad (filter read MN-major, parity-class stores), TMA-fed wgrad and the shared-memory-im2col stem, against torch
-    fp32 on bf16-rounded operands (1e-2 of the tensor maximum: bf16 output rounding)."""
+    stride-2 dgrad (filter read MN-major, parity-class stores), TMA-fed wgrad, the shared-memory-im2col stem and a stride-3
+    block through backbones._ConvBlock2D (its dgrad on csrc/conv2d_direct.cu), against torch fp32 on bf16-rounded operands
+    (1e-2 of the tensor maximum: bf16 output rounding)."""
     rows = _run_child('conv_tma_child.py')
     bad = [r for r in rows if not r.get('ok', True)]
     assert not bad, bad
     kinds = {r['kind'] for r in rows}
-    assert {'fwd', 'dgrad', 'wgrad', 'stem', 'conv3d'} <= kinds, kinds
+    assert {'fwd', 'dgrad', 'wgrad', 'stem', 'dispatch', 'conv3d'} <= kinds, kinds
 
 
 def test_union_add_and_interp_kernels():
