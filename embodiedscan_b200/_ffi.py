@@ -27,7 +27,7 @@ SIGNATURES = {
     'esb_kmap_pairs_workspace_bytes': ('iq', 'z'),
     'esb_kmap_pairs': ('piqppppzp', 'i'),
     'esb_generative_children': ('pqipp', 'i'),
-    'esb_spconv_fwd': ('ppppqiiiiiip', 'i'),
+    'esb_spconv_fwd': ('ppppqiiiiip', 'i'),
     'esb_spconv_wgrad': ('ppppppqiiiip', 'i'),
     'esb_kmap_tile_masks': ('piqpp', 'i'),
     'esb_spconv_tc_fwd': ('pppppqiiiip', 'i'),
@@ -38,12 +38,9 @@ SIGNATURES = {
     'esb_batchnorm_fwd_fused': ('ppqippfppfippip', 'i'),
     'esb_norm_apply': ('pppqippppipip', 'i'),
     'esb_norm_bwd': ('pppppiqiipppippppiip', 'i'),
-    'esb_act_fwd': ('ppqiip', 'i'),
     'esb_bias_act_fwd': ('ppppqiiip', 'i'),
     'esb_act_bwd': ('pppqiip', 'i'),
     'esb_gather2_rows': ('ppqpppqiip', 'i'),
-    'esb_head_split_fwd': ('pppqiiiifppppp', 'i'),
-    'esb_head_split_bwd': ('pppppqiiiifpppp', 'i'),
     'esb_conv2d_tma_fwd': ('ppppp' + 'iiiiiiiiii' + 'p', 'i'),
     'esb_conv2d_tma_wgrad': ('ppp' + 'iiiiiiiii' + 'p', 'i'),
     'esb_conv2d_tma_dgrad': ('ppp' + 'iiiiiiiii' + 'p', 'i'),
@@ -84,7 +81,7 @@ KERNELS_PER_CALL = {
     'esb_voxelize_points': 1, 'esb_coord_unique': 6, 'esb_hash_build': 2, 'esb_hash_lookup': 1, 'esb_kernel_map': 1,
     'esb_kernel_map_transpose': 2, 'esb_kmap_pairs': 3, 'esb_generative_children': 1, 'esb_spconv_fwd': 1,
     'esb_spconv_wgrad': 1, 'esb_maxpool_fwd': 1, 'esb_maxpool_bwd': 1, 'esb_norm_fwd': 5, 'esb_norm_apply': 1,
-    'esb_norm_bwd': 2, 'esb_batchnorm_fwd_fused': 2, 'esb_act_fwd': 1, 'esb_paint_fwd': 1, 'esb_paint_bwd': 1, 'esb_fcaf3d_targets': 5,
+    'esb_norm_bwd': 2, 'esb_batchnorm_fwd_fused': 2, 'esb_paint_fwd': 1, 'esb_paint_bwd': 1, 'esb_fcaf3d_targets': 5,
     'esb_focal_loss_fwd': 1, 'esb_focal_loss_bwd': 1, 'esb_nms_bev_segmented': 1, 'esb_iou_bev_pairwise': 1,
     'esb_img_normalize': 1, 'esb_unproject_depth': 3, 'esb_grad_clip_coef': 2, 'esb_adamw_step': 1,
     'esb_cast_f32_to_bf16': 1, 'esb_spconv_tc_fwd': 1, 'esb_spconv_tc_wgrad': 1, 'esb_kmap_tile_masks': 1,

@@ -44,10 +44,12 @@ __device__ __forceinline__ void load4<__nv_bfloat16>(const __nv_bfloat16* p, boo
 }
 
 // y[o, :] = sum_k x[nbr[k][o], :] @ W_k      (W_k = w[k] (Cin,Cout), or w[k]^T with w[k] (Cout,Cin) if WT)
+// WT (the dgrad) asks for 6 resident CTAs per SM, i.e. at most 40 registers with no spills (ptxas would take 47-48 and fit
+// 5); 0 leaves the forward instances (47 registers) to ptxas.
 template <typename T, bool WT>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, WT ? 6 : 0)
 spconv_fwd_kernel(const T* __restrict__ x, const T* __restrict__ w, const int* __restrict__ nbr, T* __restrict__ y,
-                  int n_out, int cin, int cout, int K, int accumulate) {
+                  int n_out, int cin, int cout, int K) {
   __shared__ __align__(16) float As[KC][TM + 4];
   __shared__ __align__(16) float Bs[KC][TN + 4];
   __shared__ int rows[TM];
@@ -115,12 +117,7 @@ spconv_fwd_kernel(const T* __restrict__ x, const T* __restrict__ w, const int* _
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       int col = n0 + tx * 4 + j;
-      if (col < cout) {
-        long long idx = (long long)row * cout + col;
-        float v = acc[i][j];
-        if (accumulate) v += esb_to_float<T>(y[idx]);
-        y[idx] = esb_from_float<T>(v);
-      }
+      if (col < cout) y[(long long)row * cout + col] = esb_from_float<T>(acc[i][j]);
     }
   }
 }
@@ -194,17 +191,16 @@ spconv_wgrad_kernel(const T* __restrict__ x, const T* __restrict__ dy, const int
 
 }  // namespace
 
-// x (n_in,cin), w (K,cin,cout) [or (K,cout,cin) when w_transposed], nbr (K,n_out) -> y (n_out,cout)
+// x (n_in,cin), w (K,cin,cout) [or (K,cout,cin) when w_transposed], nbr (K,n_out) -> y (n_out,cout), overwritten
 extern "C" int esb_spconv_fwd(const void* x, const void* w, const int* nbr, void* y, long long n_out, int cin, int cout,
-                              int K, int w_transposed, int accumulate, int dtype, void* stream_) {
+                              int K, int w_transposed, int dtype, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   ESB_CHECK_ARG(cin > 0 && cout > 0 && K > 0, "esb_spconv_fwd: bad channel/kernel sizes");
   ESB_CHECK_ARG(dtype == ESB_F32 || dtype == ESB_BF16, "esb_spconv_fwd: dtype must be f32 or bf16");
   if (n_out == 0) return ESB_OK;
   dim3 grid(esb_div_up(n_out, TM), esb_div_up(cout, TN));
-#define LAUNCH(T, WT)                                                                                          \
-  spconv_fwd_kernel<T, WT><<<grid, 256, 0, stream>>>((const T*)x, (const T*)w, nbr, (T*)y, (int)n_out, cin, cout, K, \
-                                                      accumulate)
+#define LAUNCH(T, WT) \
+  spconv_fwd_kernel<T, WT><<<grid, 256, 0, stream>>>((const T*)x, (const T*)w, nbr, (T*)y, (int)n_out, cin, cout, K)
   if (dtype == ESB_F32) {
     if (w_transposed) LAUNCH(float, true); else LAUNCH(float, false);
   } else {

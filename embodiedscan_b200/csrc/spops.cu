@@ -285,13 +285,6 @@ __global__ void norm_bwd_apply_kernel(const T* __restrict__ x, const T* __restri
   if (dres) dres[t] = esb_from_float<T>(g);
 }
 
-// plain activation (used where no normalisation precedes it)
-template <typename T>
-__global__ void act_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, long long n, int act) {
-  long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (t < n) y[t] = esb_from_float<T>(act_fwd(esb_to_float<T>(x[t]), act));
-}
-
 // y = act(x + bias[c] + res) over (rows, C) row-major (an NHWC activation is exactly that), 8 channels per thread.
 // Replaces cuDNN's broadcast bias add + the separate residual add + ReLU of the folded conv+BN blocks (3 passes -> 1).
 template <typename T>
@@ -584,13 +577,6 @@ extern "C" int esb_norm_bwd(const void* x, const void* y, const void* dy, const 
   return ESB_OK;
 }
 
-extern "C" int esb_act_fwd(const void* x, void* y, long long n, int act, int dtype, void* stream) {
-  if (n == 0) return ESB_OK;
-  DISPATCH_T(dtype, (act_fwd_kernel<T><<<esb_div_up(n, 256), 256, 0, (cudaStream_t)stream>>>((const T*)x, (T*)y, n, act)));
-  ESB_CUDA_LAUNCH_CHECK("act_fwd_kernel");
-  return ESB_OK;
-}
-
 // y = act(x + bias[c] + res), x/res/y (rows, C) row-major with C % 8 == 0; y may alias x. bias fp32 (C) or NULL.
 extern "C" int esb_bias_act_fwd(const void* x, const float* bias, const void* res, void* y, long long rows, int C, int act,
                                 int dtype, void* stream) {
@@ -651,135 +637,5 @@ extern "C" int esb_batchnorm_fwd_fused(const void* x, const void* res, long long
                         (const T*)x, (const T*)res, N, C, gamma, beta, eps, running_mean, running_var, momentum, act, stats,
                         (T*)y)));
   ESB_CUDA_LAUNCH_CHECK("bn_apply_fused_kernel");
-  return ESB_OK;
-}
-
-// ---------------- FCAF3D head epilogue (fcaf3d_head.py:1116-1149 after the three 1x1 convolutions) ----------------
-// `out` (N, W) bf16 is the one padded head GEMM: columns [0, n_cls) class logits without bias, column n_cls the centre-ness,
-// the next n_reg columns the box regression, the rest zero padding. One warp per row writes
-//   cls   (N, n_cls) bf16 = out + bf16(bias)                     (conv_cls bias)
-//   centre(N, 1)     fp32
-//   bbox  (N, n_reg) fp32: columns [0, n_exp) max(exp(s * x), lo) (the Scale layer, exp and clamp(min=lo)), the rest x
-//   prune (N, 1)     fp32 = max over the class logits            (the pruning score of the parent level)
-// HBM-bound: 2 B * W read + 2 B * n_cls + 4 B * (2 + n_reg) written per row.
-__global__ void __launch_bounds__(256) head_split_fwd_kernel(const __nv_bfloat16* __restrict__ out,
-                                                             const float* __restrict__ bias, const float* __restrict__ scale,
-                                                             long long N, int W, int n_cls, int n_reg, int n_exp, float lo,
-                                                             __nv_bfloat16* __restrict__ cls, float* __restrict__ centre,
-                                                             float* __restrict__ bbox, float* __restrict__ prune) {
-  const int lane = threadIdx.x & 31;
-  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
-  const float s = *scale;
-  for (long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < N; row += warps) {
-    const __nv_bfloat16* o = out + row * W;
-    float m = -INFINITY;
-    for (int c = lane; c < n_cls; c += 32) {
-      const float b = __bfloat162float(__float2bfloat16(bias[c]));
-      const __nv_bfloat16 v = __float2bfloat16(__bfloat162float(o[c]) + b);
-      cls[row * n_cls + c] = v;
-      m = fmaxf(m, __bfloat162float(v));
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, d));
-    if (lane == 0) {
-      prune[row] = m;
-      centre[row] = __bfloat162float(o[n_cls]);
-    }
-    if (lane < n_reg) {
-      const float x = __bfloat162float(o[n_cls + 1 + lane]);
-      bbox[row * n_reg + lane] = lane < n_exp ? fmaxf(expf(s * x), lo) : x;
-    }
-  }
-}
-
-// Backward of the above: dout (N, W) bf16 (padding columns zero), dbias (n_cls) += column sums of dcls, dscale += the Scale
-// gradient. clamp(min=lo) passes the gradient where exp(s x) >= lo. n_cls <= 512 (16 class columns per lane).
-__global__ void __launch_bounds__(256) head_split_bwd_kernel(const __nv_bfloat16* __restrict__ out,
-                                                             const __nv_bfloat16* __restrict__ dcls,
-                                                             const float* __restrict__ dcentre, const float* __restrict__ dbbox,
-                                                             const float* __restrict__ scale, long long N, int W, int n_cls,
-                                                             int n_reg, int n_exp, float lo, __nv_bfloat16* __restrict__ dout,
-                                                             float* __restrict__ dbias, float* __restrict__ dscale) {
-  extern __shared__ float s_bias[];                  // n_cls block-level column sums
-  const int lane = threadIdx.x & 31;
-  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
-  const float s = *scale;
-  for (int c = threadIdx.x; c < n_cls; c += blockDim.x) s_bias[c] = 0.f;
-  __syncthreads();
-  float acc[16];
-#pragma unroll
-  for (int k = 0; k < 16; ++k) acc[k] = 0.f;
-  float ds = 0.f;
-  const int used = n_cls + 1 + n_reg;
-  for (long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < N; row += warps) {
-    __nv_bfloat16* d = dout + row * W;
-#pragma unroll
-    for (int k = 0; k < 16; ++k) {
-      const int c = lane + 32 * k;
-      if (c < n_cls) {
-        const __nv_bfloat16 g = dcls[row * n_cls + c];
-        d[c] = g;
-        acc[k] += __bfloat162float(g);
-      }
-    }
-    if (lane == 0) d[n_cls] = __float2bfloat16(dcentre[row]);
-    if (lane < n_reg) {
-      float g = dbbox[row * n_reg + lane];
-      if (lane < n_exp) {
-        const float x = __bfloat162float(out[row * W + n_cls + 1 + lane]);
-        const float e = expf(s * x);
-        if (e >= lo) {
-          ds += g * e * x;
-          g = g * e * s;
-        } else {
-          g = 0.f;
-        }
-      }
-      d[n_cls + 1 + lane] = __float2bfloat16(g);
-    }
-    for (int c = used + lane; c < W; c += 32) d[c] = __float2bfloat16(0.f);
-  }
-#pragma unroll
-  for (int k = 0; k < 16; ++k) {
-    const int c = lane + 32 * k;
-    if (c < n_cls && acc[k] != 0.f) atomicAdd(&s_bias[c], acc[k]);
-  }
-#pragma unroll
-  for (int d2 = 16; d2 > 0; d2 >>= 1) ds += __shfl_xor_sync(0xffffffffu, ds, d2);
-  if (lane == 0 && ds != 0.f) atomicAdd(dscale, ds);
-  __syncthreads();
-  for (int c = threadIdx.x; c < n_cls; c += blockDim.x)
-    if (s_bias[c] != 0.f) atomicAdd(&dbias[c], s_bias[c]);
-}
-
-static int head_split_grid(long long N) {
-  long long g = esb_div_up(N, 8);                    // 8 warps (rows) per block
-  const long long cap = 4LL * esb_sm_count();
-  return (int)(g < cap ? g : cap);
-}
-
-extern "C" int esb_head_split_fwd(const void* out, const float* bias, const float* scale, long long N, int W, int n_cls,
-                                  int n_reg, int n_exp, float lo, void* cls, float* centre, float* bbox, float* prune,
-                                  void* stream) {
-  ESB_CHECK_ARG(n_cls >= 1 && n_reg >= 0 && n_reg <= 32 && n_exp <= n_reg && n_cls + 1 + n_reg <= W,
-                "esb_head_split_fwd: need n_cls >= 1, n_exp <= n_reg <= 32 and n_cls + 1 + n_reg <= W");
-  if (N == 0) return ESB_OK;
-  head_split_fwd_kernel<<<head_split_grid(N), 256, 0, (cudaStream_t)stream>>>(
-      (const __nv_bfloat16*)out, bias, scale, N, W, n_cls, n_reg, n_exp, lo, (__nv_bfloat16*)cls, centre, bbox, prune);
-  ESB_CUDA_LAUNCH_CHECK("head_split_fwd_kernel");
-  return ESB_OK;
-}
-
-// dbias (n_cls) and dscale (1) are ACCUMULATED into: the caller zeroes them.
-extern "C" int esb_head_split_bwd(const void* out, const void* dcls, const float* dcentre, const float* dbbox,
-                                  const float* scale, long long N, int W, int n_cls, int n_reg, int n_exp, float lo, void* dout,
-                                  float* dbias, float* dscale, void* stream) {
-  ESB_CHECK_ARG(n_cls >= 1 && n_cls <= 512 && n_reg >= 0 && n_reg <= 32 && n_exp <= n_reg && n_cls + 1 + n_reg <= W,
-                "esb_head_split_bwd: need 1 <= n_cls <= 512, n_exp <= n_reg <= 32 and n_cls + 1 + n_reg <= W");
-  if (N == 0) return ESB_OK;
-  head_split_bwd_kernel<<<head_split_grid(N), 256, n_cls * sizeof(float), (cudaStream_t)stream>>>(
-      (const __nv_bfloat16*)out, (const __nv_bfloat16*)dcls, dcentre, dbbox, scale, N, W, n_cls, n_reg, n_exp, lo,
-      (__nv_bfloat16*)dout, dbias, dscale);
-  ESB_CUDA_LAUNCH_CHECK("head_split_bwd_kernel");
   return ESB_OK;
 }

@@ -33,53 +33,6 @@ class Scale(nn.Module):
         return x * self.scale.to(x.dtype)
 
 
-def head_epilogue_backend() -> str:
-    """'lib' (default): the ATen slice / exp / clamp / cat chain after the head GEMM. ESB200_HEAD_EPILOGUE=own switches to the
-    fused kernel pair (esb_head_split_fwd / _bwd): checked against that chain in tests/test_kernels_gpu.py, but the
-    round's GPU time ran out before the whole training step was re-validated with it, so it is not the default yet."""
-    import os
-    return os.environ.get('ESB200_HEAD_EPILOGUE', 'lib')
-
-
-class _HeadSplit(torch.autograd.Function):
-    """Everything between the padded head GEMM and the loss (fcaf3d_head.py:1116-1149): conv_cls bias, centre-ness column,
-    Scale -> exp -> clamp(min=1e-3) on the six distances, the rest of the regression, and the row max of the class logits
-    (pruning score, not differentiable). One kernel each way instead of ~11 forward / ~15 backward ATen launches per level."""
-    N_EXP, LO = 6, 1e-3
-
-    @staticmethod
-    def forward(ctx, out, bias, scale, n_cls, n_reg):
-        out = out.contiguous()
-        N, W = out.shape
-        bias32 = bias.detach().float().reshape(-1).contiguous()
-        scale32 = scale.detach().float().reshape(1).contiguous()
-        cls = out.new_empty(N, n_cls)
-        centre = torch.empty(N, 1, dtype=torch.float32, device=out.device)
-        bbox = torch.empty(N, n_reg, dtype=torch.float32, device=out.device)
-        score = torch.empty(N, 1, dtype=torch.float32, device=out.device)
-        call('esb_head_split_fwd', ptr(out), ptr(bias32), ptr(scale32), N, W, n_cls, n_reg, min(_HeadSplit.N_EXP, n_reg),
-             _HeadSplit.LO, ptr(cls), ptr(centre), ptr(bbox), ptr(score), stream())
-        ctx.save_for_backward(out, scale32)
-        ctx.dims = (n_cls, n_reg, bias.dtype, tuple(bias.shape), scale.dtype, tuple(scale.shape))
-        ctx.mark_non_differentiable(score)
-        return cls, centre, bbox, score
-
-    @staticmethod
-    def backward(ctx, dcls, dcentre, dbbox, _dscore):
-        out, scale32 = ctx.saved_tensors
-        n_cls, n_reg, bias_dtype, bias_shape, scale_dtype, scale_shape = ctx.dims
-        N, W = out.shape
-        dcls = dcls.to(out.dtype).contiguous()
-        dcentre = dcentre.float().contiguous()
-        dbbox = dbbox.float().contiguous()
-        dout = torch.empty_like(out)
-        acc = torch.zeros(n_cls + 1, dtype=torch.float32, device=out.device)      # [dbias | dscale]
-        call('esb_head_split_bwd', ptr(out), ptr(dcls), ptr(dcentre), ptr(dbbox), ptr(scale32), N, W, n_cls, n_reg,
-             min(_HeadSplit.N_EXP, n_reg), _HeadSplit.LO, ptr(dout), ptr(acc), acc.data_ptr() + 4 * n_cls, stream())
-        return (dout, acc[:n_cls].reshape(bias_shape).to(bias_dtype), acc[n_cls].reshape(scale_shape).to(scale_dtype), None,
-                None)
-
-
 @MODELS.register_module()
 class BBoxCDLoss(nn.Module):
     """embodiedscan/models/losses/chamfer_distance.py:206-285 (mode 'l1', group 'g8', src->dst only)."""
@@ -395,19 +348,14 @@ class FCAF3DHeadRotMat(nn.Module):
                           self.conv_cls.kernel.new_zeros(self.conv_cls.kernel.shape[0], width - n_cls - 1 - n_reg)], 1)
 
     def _forward_single_level(self, x: SP.SparseTensor, scale: Scale, need_prune_score: bool = True, w_all=None):
-        """_forward_single (fcaf3d_head.py:1116-1149) on whole-batch rows: one GEMM for the three 1x1 heads, one kernel for
-        everything after it (bias, Scale, exp, clamp, the column split and the pruning score)."""
+        """_forward_single (fcaf3d_head.py:1116-1149) on whole-batch rows: bf16 features with a multiple of 64 channels take
+        one GEMM for the three 1x1 heads (rows_gemm), other rows one product for cls and one for centre + reg. Everything after
+        the products (bias, Scale, exp, clamp, the column split and the pruning score) is ATen."""
         f = x.F
         coords = x.C
         n_cls, n_reg = self.conv_cls.kernel.shape[1], self.conv_reg.kernel.shape[1]
         if f.is_cuda and f.dtype == torch.bfloat16 and f.shape[1] % 64 == 0:
             out = SP.rows_gemm(f, (self._head_weights(f) if w_all is None else w_all).to(f.dtype))
-            if head_epilogue_backend() == 'own' and n_cls <= 512 and n_reg <= 32:
-                cls_pred, center_pred, bbox_pred, score = _HeadSplit.apply(out, self.conv_cls.bias, scale.scale, n_cls, n_reg)
-                prune_scores = x.replace_feature(score) if need_prune_score else None
-                lv = dict(center=center_pred, bbox=bbox_pred, cls=cls_pred, points=coords[:, 1:] * self.voxel_size,
-                          batch=coords[:, 0].contiguous(), tensor=x)
-                return lv, prune_scores
             cls_pred = out[:, :n_cls] + self.conv_cls.bias.to(f.dtype)
             small = out[:, n_cls:n_cls + 1 + n_reg].float()
         else:

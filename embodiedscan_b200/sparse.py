@@ -24,10 +24,6 @@ from ._ffi import call, ptr, query, stream
 
 ACT_NONE, ACT_RELU, ACT_ELU = 0, 1, 2
 
-# bf16 sparse convolutions run on the wgmma tensor-core kernels when the channel counts tile (multiples of 64)
-USE_TENSOR_CORES = True
-USE_TC_WGRAD = True
-
 # bench.py switches this on to time every sparse-conv launch with CUDA events on the launching stream
 CONV_PROFILE = {'enabled': False, 'records': []}
 
@@ -282,13 +278,14 @@ class _SparseConv(torch.autograd.Function):
         # bf16: the arena's shadow copy when it mirrors the current value (engine.py), else a fresh cast
         w = bf16_operand(weight) if x.dtype == torch.bfloat16 else weight.detach().to(x.dtype).contiguous()
         y = torch.empty((kmap.n_out, cout), dtype=x.dtype, device=x.device)
-        tc = USE_TENSOR_CORES and x.dtype == torch.bfloat16 and cin % 64 == 0 and cout % 64 == 0
+        # bf16 sparse convolutions run on the wgmma tensor-core kernels when the channel counts tile (multiples of 64)
+        tc = x.dtype == torch.bfloat16 and cin % 64 == 0 and cout % 64 == 0
         if tc:   # the stored (K,cin,cout) kernel is the MN-major B operand: no transpose copy
             _timed_conv_call('fwd', kmap, cin, cout, x.dtype, 'esb_spconv_tc_fwd', ptr(x), ptr(w), ptr(kmap.nbr_out),
                              ptr(kmap.tile_masks('out')), ptr(y), kmap.n_out, cin, cout, K, 1, stream())
         else:
             _timed_conv_call('fwd', kmap, cin, cout, x.dtype, 'esb_spconv_fwd', ptr(x), ptr(w), ptr(kmap.nbr_out),
-                             ptr(y), kmap.n_out, cin, cout, K, 0, 0, _ffi.dtype_code(x.dtype), stream())
+                             ptr(y), kmap.n_out, cin, cout, K, 0, _ffi.dtype_code(x.dtype), stream())
         ctx.save_for_backward(x, w)
         ctx.kmap, ctx.cin, ctx.cout, ctx.wshape, ctx.tc, ctx.weight = kmap, cin, cout, weight.shape, tc, weight
         if ctx.needs_input_grad[1]:
@@ -310,14 +307,14 @@ class _SparseConv(torch.autograd.Function):
                                  ptr(kmap.tile_masks('in')), ptr(dx), kmap.n_in, cout, cin, kmap.K, 0, stream())
             else:
                 _timed_conv_call('dgrad', kmap, cout, cin, x.dtype, 'esb_spconv_fwd', ptr(dy), ptr(w), ptr(kmap.nbr_in),
-                                 ptr(dx), kmap.n_in, cout, cin, kmap.K, 1, 0, code, stream())
+                                 ptr(dx), kmap.n_in, cout, cin, kmap.K, 1, code, stream())
         if ctx.needs_input_grad[1]:
             pin, pout, koff, tot = kmap.pairs
             weight = ctx.weight
             direct = getattr(weight, '_esb_grad_direct', False) and weight.grad is not None
             # arena parameters: the kernel accumulates straight into the flat gradient buffer (no zeros + add_ pass)
             dw = weight.grad if direct else torch.zeros((kmap.K, cin, cout), dtype=torch.float32, device=x.device)
-            if ctx.tc and USE_TC_WGRAD:
+            if ctx.tc:
                 _timed_conv_call('wgrad', kmap, cin, cout, x.dtype, 'esb_spconv_tc_wgrad', ptr(x), ptr(dy), ptr(pin),
                                  ptr(pout), ptr(koff), ptr(dw), tot, cin, cout, kmap.K, stream())
             else:
@@ -410,7 +407,7 @@ class _RowsGemmTC(torch.autograd.Function):
 def rows_gemm(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
     """x (N, cin) @ w (cin, cout). bf16 CUDA rows with channel counts that tile (multiples of 64) run on the library's
     tensor-core kernels; anything else (fp32 parity arithmetic, odd widths) is a plain matmul."""
-    if (USE_TENSOR_CORES and x.is_cuda and x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.shape[1] % 64 == 0
+    if (x.is_cuda and x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.shape[1] % 64 == 0
             and w.shape[1] % 64 == 0):
         return _RowsGemmTC.apply(x, w)
     return x @ w.to(x.dtype)

@@ -60,7 +60,7 @@ int esb_generative_children(const int* coords_in, long long n_in, int half_strid
 
 /* ---- sparse convolution (ME.MinkowskiConvolution fwd/bwd; mink_resnet.py:58-62, fcaf3d_head.py:919-946) -------- */
 int esb_spconv_fwd(const void* x, const void* w, const int* nbr, void* y, long long n_out, int cin, int cout, int K,
-                   int w_transposed, int accumulate, int dtype, void* stream);
+                   int w_transposed, int dtype, void* stream);
 int esb_spconv_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out, const int* k_offsets,
                      float* dw, long long n_pairs_hint, int cin, int cout, int K, int dtype, void* stream);
 
@@ -86,20 +86,11 @@ int esb_norm_fwd(const void* x, const void* res, const int* seg_off, const int* 
 int esb_batchnorm_fwd_fused(const void* x, const void* res, long long N, int C, const float* gamma, const float* beta, float eps,
                             float* running_mean, float* running_var, float momentum, int act, float* stats, void* y, int dtype,
                             void* stream);
-/* FCAF3D head epilogue (replaces the slice / bias / Scale / exp / clamp / cat chain of fcaf3d_head.py:1116-1149 applied to the
- * one padded head GEMM `out` (N, W) bf16 = [cls n_cls | centre 1 | reg n_reg | zero pad]): cls (N, n_cls) bf16 with the conv_cls
- * bias, centre (N, 1) fp32, bbox (N, n_reg) fp32 whose first n_exp columns are max(exp(scale * x), lo), prune (N, 1) fp32 = row
- * max of cls. The backward accumulates dbias (n_cls) and dscale (1) into caller-zeroed buffers and writes dout (N, W) bf16. */
-int esb_head_split_fwd(const void* out, const float* bias, const float* scale, long long N, int W, int n_cls, int n_reg, int n_exp,
-                       float lo, void* cls, float* centre, float* bbox, float* prune, void* stream);
-int esb_head_split_bwd(const void* out, const void* dcls, const float* dcentre, const float* dbbox, const float* scale, long long N,
-                       int W, int n_cls, int n_reg, int n_exp, float lo, void* dout, float* dbias, float* dscale, void* stream);
 int esb_norm_apply(const void* x, const void* res, const int* row_seg, long long N, int C, const float* mean,
                    const float* rstd, const float* gamma, const float* beta, int act, void* y, int dtype, void* stream);
 int esb_norm_bwd(const void* x, const void* y, const void* dy, const int* seg_off, const int* row_seg, int S,
                  long long N, int max_seg_rows, int C, const float* mean, const float* rstd, const float* gamma, int act,
                  float* sg, float* sgx, void* dx, void* dres, int zero_sums, int dtype, void* stream);
-int esb_act_fwd(const void* x, void* y, long long n, int act, int dtype, void* stream);
 /* fused epilogue of the folded conv+BN blocks of the per-view 2D ResNet: y = act(x + bias[c] + res) on NHWC rows */
 int esb_bias_act_fwd(const void* x, const float* bias, const void* res, void* y, long long rows, int C, int act,
                      int dtype, void* stream);

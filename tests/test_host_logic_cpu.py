@@ -242,86 +242,3 @@ def test_train_step_log_vars_carry_no_autograd_history():
     assert set(out) == set(log_vars)
     assert all(v.grad_fn is None and not v.requires_grad for v in out.values())
     assert float(out['loss']) == float(loss) == 6 + 9 + 12
-
-
-def _host_view(address, shape, dtype):
-    """A torch tensor over raw host memory (the emulated kernels below read and write through the pointers they are given)."""
-    n = int(np.prod(shape))
-    if n == 0:
-        return torch.empty(shape, dtype=dtype)
-    ctype = {torch.float32: ctypes.c_float, torch.bfloat16: ctypes.c_uint16}[dtype]
-    arr = np.ctypeslib.as_array((ctype * n).from_address(address))
-    t = torch.from_numpy(arr)
-    return (t.view(torch.bfloat16) if dtype == torch.bfloat16 else t).reshape(shape)
-
-
-def test_head_epilogue_function_plumbing_with_model_shaped_parameters(monkeypatch):
-    """dense_heads._HeadSplit around an emulation of esb_head_split_fwd / _bwd that works through the raw pointers: the host
-    side (buffer shapes, (1, n_cls) bias and 0-dim Scale parameters as the model holds them, gradient shapes and dtypes,
-    non-differentiable pruning score) against the ATen chain of fcaf3d_head.py:1116-1149. The kernels themselves are checked
-    on the GPU (tests/test_kernels_gpu.py)."""
-    from embodiedscan_b200 import dense_heads as DH
-
-    def fake_call(name, *a):
-        if name == 'esb_head_split_fwd':
-            out_p, bias_p, scale_p, N, W, n_cls, n_reg, n_exp, lo, cls_p, ctr_p, box_p, score_p, _ = a
-            out = _host_view(out_p, (N, W), torch.bfloat16).float()
-            bias = _host_view(bias_p, (n_cls, ), torch.float32).bfloat16().float()
-            s = _host_view(scale_p, (1, ), torch.float32)[0]
-            cls = (out[:, :n_cls] + bias).bfloat16()
-            _host_view(cls_p, (N, n_cls), torch.bfloat16).copy_(cls)
-            _host_view(ctr_p, (N, 1), torch.float32).copy_(out[:, n_cls:n_cls + 1])
-            reg = out[:, n_cls + 1:n_cls + 1 + n_reg]
-            _host_view(box_p, (N, n_reg), torch.float32).copy_(
-                torch.cat((torch.exp(reg[:, :n_exp] * s).clamp(min=lo), reg[:, n_exp:]), 1))
-            _host_view(score_p, (N, 1), torch.float32).copy_(cls.float().max(1, keepdim=True).values)
-        elif name == 'esb_head_split_bwd':
-            out_p, dcls_p, dctr_p, dbox_p, scale_p, N, W, n_cls, n_reg, n_exp, lo, dout_p, dbias_p, dscale_p, _ = a
-            out = _host_view(out_p, (N, W), torch.bfloat16).float()
-            s = _host_view(scale_p, (1, ), torch.float32)[0]
-            dcls = _host_view(dcls_p, (N, n_cls), torch.bfloat16)
-            dbox = _host_view(dbox_p, (N, n_reg), torch.float32).clone()
-            x = out[:, n_cls + 1:n_cls + 1 + n_exp]
-            e = torch.exp(x * s)
-            live = (e >= lo).float()
-            _host_view(dscale_p, (1, ), torch.float32).add_((dbox[:, :n_exp] * e * x * live).sum())
-            dbox[:, :n_exp] *= e * s * live
-            dout = _host_view(dout_p, (N, W), torch.bfloat16)
-            dout.zero_()
-            dout[:, :n_cls] = dcls
-            dout[:, n_cls:n_cls + 1] = _host_view(dctr_p, (N, 1), torch.float32).bfloat16()
-            dout[:, n_cls + 1:n_cls + 1 + n_reg] = dbox.bfloat16()
-            _host_view(dbias_p, (n_cls, ), torch.float32).add_(dcls.float().sum(0))
-        else:
-            raise AssertionError(name)
-
-    monkeypatch.setattr(DH, 'call', fake_call)
-    monkeypatch.setattr(DH, 'stream', lambda: None)
-    torch.manual_seed(3)
-    N, n_cls, n_reg, W = 53, 18, 12, 64
-    out = (torch.randn(N, W) * 2).bfloat16()
-    out[:9, n_cls + 1:n_cls + 7] -= 30.0
-    bias = torch.randn(1, n_cls)                     # MinkowskiConvolution bias layout
-    scale = torch.tensor(0.7)                        # mmcv Scale: 0-dim
-    g_cls, g_ctr, g_box = torch.randn(N, n_cls).bfloat16(), torch.randn(N, 1), torch.randn(N, n_reg)
-
-    o1, b1, s1 = out.clone().requires_grad_(True), bias.clone().requires_grad_(True), scale.clone().requires_grad_(True)
-    cls, ctr, box, score = DH._HeadSplit.apply(o1, b1, s1, n_cls, n_reg)
-    assert cls.dtype == torch.bfloat16 and ctr.dtype == box.dtype == score.dtype == torch.float32
-    assert not score.requires_grad and cls.requires_grad and box.requires_grad
-    (cls.float() * g_cls.float()).sum().add((ctr * g_ctr).sum()).add((box * g_box).sum()).backward()
-
-    o2, b2, s2 = out.clone().requires_grad_(True), bias.clone().requires_grad_(True), scale.clone().requires_grad_(True)
-    cls_r = o2[:, :n_cls] + b2.to(o2.dtype)
-    small = o2[:, n_cls:n_cls + 1 + n_reg].float()
-    reg = small[:, 1:]
-    box_r = torch.cat((torch.exp(reg[:, :6] * s2).clamp(min=1e-3), reg[:, 6:]), 1)
-    (cls_r.float() * g_cls.float()).sum().add((small[:, :1] * g_ctr).sum()).add((box_r * g_box).sum()).backward()
-
-    assert torch.equal(cls, cls_r) and torch.equal(ctr, small[:, :1]) and torch.equal(box, box_r)
-    assert torch.equal(score, cls_r.max(1, keepdim=True).values.float())
-    assert b1.grad.shape == bias.shape and s1.grad.shape == scale.shape and o1.grad.shape == out.shape
-    assert b1.grad.dtype == torch.float32 and o1.grad.dtype == torch.bfloat16
-    assert torch.equal(o1.grad, o2.grad)
-    assert float((b1.grad - b2.grad).abs().max()) <= 2e-2 * float(b2.grad.abs().max())      # reference sums in bf16
-    assert float((s1.grad - s2.grad).abs()) <= 1e-4 * float(s2.grad.abs())
