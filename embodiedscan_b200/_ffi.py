@@ -61,7 +61,9 @@ SIGNATURES = {
     'esb_fcaf3d_targets': ('ppiippppp' + 'iiiii' + 'pppp' + 'pzp', 'i'),
     'esb_focal_loss_fwd': ('ppqiffppip', 'i'),
     'esb_focal_loss_bwd': ('ppqiffpppip', 'i'),
-    'esb_bbox_cd_loss': ('pppppippp', 'i'),
+    'esb_bbox_cd_loss': ('ppppp' + 'iiii' + 'ppp', 'i'),
+    'esb_chamfer_fwd': ('pp' + 'iiiii' + 'ppppp', 'i'),
+    'esb_chamfer_bwd': ('pppppp' + 'iiiii' + 'ppp', 'i'),
     'esb_nms_bev_segmented': ('ppiifipp', 'i'),
     'esb_iou_bev_pairwise': ('pipiipp', 'i'),
     'esb_box3d_overlap': ('pipippp', 'i'),
@@ -85,6 +87,7 @@ KERNELS_PER_CALL = {
     'esb_focal_loss_fwd': 1, 'esb_focal_loss_bwd': 1, 'esb_nms_bev_segmented': 1, 'esb_iou_bev_pairwise': 1,
     'esb_img_normalize': 1, 'esb_unproject_depth': 3, 'esb_grad_clip_coef': 2, 'esb_adamw_step': 1,
     'esb_cast_f32_to_bf16': 1, 'esb_spconv_tc_fwd': 1, 'esb_spconv_tc_wgrad': 1, 'esb_kmap_tile_masks': 1,
+    'esb_chamfer_fwd': 2, 'esb_chamfer_bwd': 4,
 }
 launch_counter = {'kernels': 0, 'calls': 0, 'by_name': {}}
 

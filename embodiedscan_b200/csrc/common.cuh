@@ -51,6 +51,31 @@ int esb_sum_partial_rows(const float* part, int n_parts, long long width, float*
 // streaming multiprocessors of the current device (grid sizing; read once per device)
 int esb_sm_count();
 
+// ---- chamfer criteria (ESB_CD_*), per coordinate: torch l1_loss / mse_loss / smooth_l1_loss(beta=1), reduction none --
+// The products are rounded on their own (no FMA contraction), as ATen rounds them, so nearest-neighbour choices agree.
+template <int MODE>
+__device__ __forceinline__ float esb_cd_crit(float x) {
+  if constexpr (MODE == ESB_CD_L1) {
+    return fabsf(x);
+  } else if constexpr (MODE == ESB_CD_L2) {
+    return __fmul_rn(x, x);
+  } else {
+    const float a = fabsf(x);
+    return a < 1.f ? __fmul_rn(0.5f * a, a) : a - 0.5f;
+  }
+}
+// derivative of esb_cd_crit: sign(x) with sign(0) = 0, 2x, x clamped to [-1, 1]
+template <int MODE>
+__device__ __forceinline__ float esb_cd_dcrit(float x) {
+  if constexpr (MODE == ESB_CD_L1) {
+    return x > 0.f ? 1.f : (x < 0.f ? -1.f : 0.f);
+  } else if constexpr (MODE == ESB_CD_L2) {
+    return 2.f * x;
+  } else {
+    return fminf(fmaxf(x, -1.f), 1.f);
+  }
+}
+
 
 // ---- coordinate key packing: [b:16 | x:16 | y:16 | z:16], xyz biased by 2^15 ----
 #define ESB_EMPTY_KEY 0xFFFFFFFFFFFFFFFFull

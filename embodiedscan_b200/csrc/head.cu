@@ -282,7 +282,7 @@ __global__ void focal_bwd_kernel(const T* __restrict__ logits, const long long* 
 // One thread per positive location. Replaces, for the positives of the whole batch, _bbox_pred_to_bbox
 // (fcaf3d_head.py:1454-1525: 6 face distances + 6D rotation -> centre/size/Euler ZXY), ortho_6d_2_Mat (:1739-1750),
 // pytorch3d matrix_to_euler_angles / euler_angles_to_matrix ('ZXY'), bbox_to_corners (chamfer_distance.py:160-203) and
-// the four decoupled BBoxCDLoss terms (fcaf3d_head.py:1224-1281; L1 chamfer, src->dst only) — ~600 tiny launches of
+// the four decoupled BBoxCDLoss terms (fcaf3d_head.py:1224-1281; l1 / l2 / smooth-L1 chamfer, src->dst only) — ~600 tiny launches of
 // autograd ops in the reference formulation. The gradient w.r.t. the 12 regression channels is carried by forward-mode
 // dual numbers, so the backward pass is a single scale of the stored gradient.
 struct Dual {
@@ -385,7 +385,9 @@ __device__ __forceinline__ void euler_to_mat_f(float a, float b, float c, float 
   m[3] = a10 * cc - a12 * sc; m[4] = a11; m[5] = a10 * sc + a12 * cc;
   m[6] = -a22 * sc;           m[7] = a21; m[8] = a22 * cc;
 }
-// sum over the 8 corners of min_j L1(src corner, dst corner j); src = (centre, size, euler) duals, dst precomputed
+// sum over the 8 corners of min_j dist(src corner, dst corner j), dist = sum over x, y, z of the MODE criterion;
+// GROUP 4 restricts corners 0-3 and 4-7 to their own half of dst. src = (centre, size, euler) duals, dst precomputed.
+template <int MODE, int GROUP>
 __device__ Dual corner_chamfer(const Dual ctr[3], const Dual size[3], const Dual eul[3], const float dst[24]) {
   Dual m[9];
   euler_to_mat(eul[0], eul[1], eul[2], m);
@@ -398,14 +400,23 @@ __device__ Dual corner_chamfer(const Dual ctr[3], const Dual size[3], const Dual
     Dual cy = ctr[1] + (hx * m[3] + hy * m[4] + hz * m[5]);
     Dual cz = ctr[2] + (hx * m[6] + hy * m[7] + hz * m[8]);
     float best = INFINITY;
-    int bj = 0;
-    for (int j = 0; j < 8; ++j) {
-      float dsum = fabsf(cx.v - dst[3 * j]) + fabsf(cy.v - dst[3 * j + 1]) + fabsf(cz.v - dst[3 * j + 2]);
-      if (dsum < best) { best = dsum; bj = j; }
+    const int j0 = GROUP == 4 ? (i & 4) : 0;
+    int bj = j0;
+    for (int j = j0; j < j0 + GROUP; ++j) {
+      float dsum = esb_cd_crit<MODE>(cx.v - dst[3 * j]) + esb_cd_crit<MODE>(cy.v - dst[3 * j + 1]) +
+                   esb_cd_crit<MODE>(cz.v - dst[3 * j + 2]);
+      if (dsum < best) { best = dsum; bj = j; }      // strict: the lowest index wins ties, as torch.min
     }
-    float gx = cx.v > dst[3 * bj] ? 1.f : (cx.v < dst[3 * bj] ? -1.f : 0.f);
-    float gy = cy.v > dst[3 * bj + 1] ? 1.f : (cy.v < dst[3 * bj + 1] ? -1.f : 0.f);
-    float gz = cz.v > dst[3 * bj + 2] ? 1.f : (cz.v < dst[3 * bj + 2] ? -1.f : 0.f);
+    float gx, gy, gz;
+    if constexpr (MODE == ESB_CD_L1) {
+      gx = cx.v > dst[3 * bj] ? 1.f : (cx.v < dst[3 * bj] ? -1.f : 0.f);
+      gy = cy.v > dst[3 * bj + 1] ? 1.f : (cy.v < dst[3 * bj + 1] ? -1.f : 0.f);
+      gz = cz.v > dst[3 * bj + 2] ? 1.f : (cz.v < dst[3 * bj + 2] ? -1.f : 0.f);
+    } else {
+      gx = esb_cd_dcrit<MODE>(cx.v - dst[3 * bj]);
+      gy = esb_cd_dcrit<MODE>(cy.v - dst[3 * bj + 1]);
+      gz = esb_cd_dcrit<MODE>(cz.v - dst[3 * bj + 2]);
+    }
     total.v += best;
 #pragma unroll
     for (int q = 0; q < 12; ++q) total.d[q] += gx * cx.d[q] + gy * cy.d[q] + gz * cz.d[q];
@@ -413,6 +424,8 @@ __device__ Dual corner_chamfer(const Dual ctr[3], const Dual size[3], const Dual
   return total;
 }
 
+// NORM: the three decoupled terms of a row are divided by clamp(|target size|, 0.1) (fcaf3d_head.py:1229-1253).
+template <int MODE, int GROUP, bool NORM>
 __global__ void __launch_bounds__(64)
 bbox_cd_loss_kernel(const float* __restrict__ points, const float* __restrict__ bbox_pred, const float* __restrict__ tgt,
                     const float* __restrict__ row_w, float w0, float w1, float w2, float w3, int P,
@@ -456,10 +469,11 @@ bbox_cd_loss_kernel(const float* __restrict__ points, const float* __restrict__ 
     Dual ts[3] = {dconst(t[3]), dconst(t[4]), dconst(t[5])};
     Dual te[3] = {dconst(t[6]), dconst(t[7]), dconst(t[8])};
     Dual acc = dconst(0.f);
-    if (w0 != 0.f) acc = acc + corner_chamfer(pc, ts, te, dst) * w0;
-    if (w1 != 0.f) acc = acc + corner_chamfer(tc, ps, te, dst) * w1;
-    if (w2 != 0.f) acc = acc + corner_chamfer(tc, ts, eul, dst) * w2;
-    if (w3 != 0.f) acc = acc + corner_chamfer(pc, ps, eul, dst) * w3;
+    if (w0 != 0.f) acc = acc + corner_chamfer<MODE, GROUP>(pc, ts, te, dst) * w0;
+    if (w1 != 0.f) acc = acc + corner_chamfer<MODE, GROUP>(tc, ps, te, dst) * w1;
+    if (w2 != 0.f) acc = acc + corner_chamfer<MODE, GROUP>(tc, ts, eul, dst) * w2;
+    if constexpr (NORM) acc = acc * (1.f / fmaxf(sqrtf(t[3] * t[3] + t[4] * t[4] + t[5] * t[5]), 0.1f));
+    if (w3 != 0.f) acc = acc + corner_chamfer<MODE, GROUP>(pc, ps, eul, dst) * w3;
     float w = row_w[p];
     lval = acc.v * w;
 #pragma unroll
@@ -550,18 +564,32 @@ extern "C" int esb_focal_loss_bwd(const void* logits, const long long* target, l
   return ESB_OK;
 }
 
+using BboxCdKernel = void (*)(const float*, const float*, const float*, const float*, float, float, float, float, int,
+                              float*, float*);
+template <int MODE>
+static BboxCdKernel bbox_cd_pick(int group, int norm) {
+  if (group == 8) return norm ? bbox_cd_loss_kernel<MODE, 8, true> : bbox_cd_loss_kernel<MODE, 8, false>;
+  return norm ? bbox_cd_loss_kernel<MODE, 4, true> : bbox_cd_loss_kernel<MODE, 4, false>;
+}
+
 // Fused decode + decoupled corner-chamfer box loss over P positives:
-//   loss_out (device fp32, accumulated; caller zeroes) = sum_p row_w[p] * sum_v w[v] * sum_{8 corners} min_j L1
+//   loss_out (device fp32, accumulated; caller zeroes) = sum_p row_w[p] * sum_v w[v] * sum_{8 corners} min_j dist
 //   grad (P,12) = d loss / d bbox_pred. Variants v: (pred centre), (pred size), (pred euler), (all predicted).
 extern "C" int esb_bbox_cd_loss(const float* points, const float* bbox_pred, const float* targets, const float* row_w,
-                                const float* w4_host, int P, float* loss_out, float* grad, void* stream) {
+                                const float* w4_host, int P, int mode, int group, int norm_decouple, float* loss_out,
+                                float* grad, void* stream) {
+  ESB_CHECK_ARG(mode == ESB_CD_L1 || mode == ESB_CD_L2 || mode == ESB_CD_SMOOTH_L1, "esb_bbox_cd_loss: bad mode %d", mode);
+  ESB_CHECK_ARG(group == 8 || group == 4, "esb_bbox_cd_loss: group must be 8 or 4, got %d", group);
   if (P == 0) return ESB_OK;
   cudaStream_t s = (cudaStream_t)stream;
+  const BboxCdKernel kernel = mode == ESB_CD_L1 ? bbox_cd_pick<ESB_CD_L1>(group, norm_decouple)
+                              : mode == ESB_CD_L2 ? bbox_cd_pick<ESB_CD_L2>(group, norm_decouple)
+                                                  : bbox_cd_pick<ESB_CD_SMOOTH_L1>(group, norm_decouple);
   const int grid = esb_div_up(P, 64);
   float* part = nullptr;
   ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, (size_t)grid * sizeof(float), s));
-  bbox_cd_loss_kernel<<<grid, 64, 0, s>>>(points, bbox_pred, targets, row_w, w4_host[0], w4_host[1], w4_host[2], w4_host[3], P,
-                                          part, grad);
+  kernel<<<grid, 64, 0, s>>>(points, bbox_pred, targets, row_w, w4_host[0], w4_host[1], w4_host[2], w4_host[3], P, part,
+                             grad);
   ESB_CUDA_LAUNCH_CHECK("bbox_cd_loss_kernel");
   int rc = esb_sum_partial_rows(part, grid, 1, loss_out, 1, s);
   ESB_CUDA_CALL(esb_scratch_free(part, s));

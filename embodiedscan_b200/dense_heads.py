@@ -16,8 +16,8 @@ import torch.nn.functional as F
 from . import _ffi
 from . import sparse as SP
 from ._ffi import call, ptr, query, stream
-from .geometry import (bbox_cd_loss, bbox_to_corners, chamfer_l1_src, euler_angles_to_matrix,
-                       matrix_to_euler_angles_zxy, ortho_6d_2_mat, rotation_3d_in_euler)
+from .geometry import (CD_GROUPS, CD_MODES, CD_REDUCTIONS, bbox_cd_loss, bbox_to_corners, chamfer_src,
+                       euler_angles_to_matrix, matrix_to_euler_angles_zxy, ortho_6d_2_mat, rotation_3d_in_euler)
 from .registry import MODELS
 from .structures import EulerDepthInstance3DBoxes, InstanceData
 
@@ -33,17 +33,123 @@ class Scale(nn.Module):
         return x * self.scale.to(x.dtype)
 
 
+def _check_cd_options(mode=None, group=None, reduction=None):
+    for value, valid, what in ((mode, CD_MODES, 'mode'), (group, CD_GROUPS, 'group'), (reduction, CD_REDUCTIONS, 'reduction')):
+        if value is not None and value not in valid:
+            raise ValueError(f'chamfer {what} must be one of {valid}, got {value!r}')
+
+
+def check_head_box_loss(loss):
+    """A head averages its box loss itself, so the loss module must keep reduction='mean' (the reference's heads stack
+    per-scan 'sum' / 'none' results into values that are not a loss)."""
+    reduction = getattr(loss, 'reduction', 'mean')
+    if reduction != 'mean':
+        raise ValueError(f"the box loss of a head supports reduction='mean' only, got reduction={reduction!r}")
+
+
 @MODELS.register_module()
 class BBoxCDLoss(nn.Module):
-    """embodiedscan/models/losses/chamfer_distance.py:206-285 (mode 'l1', group 'g8', src->dst only)."""
+    """embodiedscan/models/losses/chamfer_distance.py:206-285: chamfer distance from the 8 corners of each source box
+    to the corners of its target box (src->dst only), criterion 'l1' / 'l2' / 'smooth_l1', corner groups 'g8' / 'g4'."""
 
     def __init__(self, mode='l2', group='g8', reduction='mean', loss_weight=1.0):
         super().__init__()
-        assert mode == 'l1' and group == 'g8' and reduction == 'mean', 'hot-path configuration: l1 / g8 / mean'
+        _check_cd_options(mode, group, reduction)
         self.mode, self.group, self.reduction, self.loss_weight = mode, group, reduction, loss_weight
 
-    def forward(self, source, target, **kwargs):
-        return bbox_cd_loss(source, target, self.loss_weight)
+    def forward(self, source, target, loss_weight=1.0, reduction_override=None, **kwargs):
+        _check_cd_options(reduction=reduction_override)
+        reduction = reduction_override if reduction_override else self.reduction
+        return bbox_cd_loss(source, target, self.loss_weight, self.mode, self.group, reduction, loss_weight)
+
+
+_CD_MODE_CODE = {'l1': 0, 'l2': 1, 'smooth_l1': 2}     # ESB_CD_L1 / ESB_CD_L2 / ESB_CD_SMOOTH_L1
+
+
+class _ChamferNN(torch.autograd.Function):
+    """csrc/chamfer.cu: nearest-neighbour distances in both directions (dist1 (B,N), dist2 (B,M)) and their int64
+    arg-minima; backward maps d/d dist1 and d/d dist2 to the points, deterministically."""
+
+    @staticmethod
+    def forward(ctx, src, dst, mode):
+        s, d = src.float().contiguous(), dst.float().contiguous()
+        B, N, C = s.shape
+        M = d.shape[1]
+        dev = s.device
+        dist1 = torch.empty((B, N), dtype=torch.float32, device=dev)
+        dist2 = torch.empty((B, M), dtype=torch.float32, device=dev)
+        idx1 = torch.empty((B, N), dtype=torch.int64, device=dev)
+        idx2 = torch.empty((B, M), dtype=torch.int64, device=dev)
+        call('esb_chamfer_fwd', ptr(s), ptr(d), B, N, M, C, _CD_MODE_CODE[mode], ptr(dist1), ptr(dist2), ptr(idx1),
+             ptr(idx2), stream())
+        ctx.save_for_backward(s, d, idx1, idx2)
+        ctx.mode, ctx.dtypes = mode, (src.dtype, dst.dtype)
+        ctx.mark_non_differentiable(idx1, idx2)
+        return dist1, dist2, idx1, idx2
+
+    @staticmethod
+    def backward(ctx, g1, g2, _g_idx1, _g_idx2):
+        s, d, idx1, idx2 = ctx.saved_tensors
+        B, N, C = s.shape
+        M = d.shape[1]
+        g1 = None if g1 is None else g1.float().contiguous()
+        g2 = None if g2 is None else g2.float().contiguous()
+        grad_src, grad_dst = torch.empty_like(s), torch.empty_like(d)
+        call('esb_chamfer_bwd', ptr(s), ptr(d), ptr(idx1), ptr(idx2), ptr(g1), ptr(g2), B, N, M, C,
+             _CD_MODE_CODE[ctx.mode], ptr(grad_src), ptr(grad_dst), stream())
+        return grad_src.to(ctx.dtypes[0]), grad_dst.to(ctx.dtypes[1]), None
+
+
+def chamfer_distance(src, dst, src_weight=1.0, dst_weight=1.0, criterion_mode='l2', reduction='mean'):
+    """chamfer_distance.py:13-79 on csrc/chamfer.cu. src (B,N,C), dst (B,M,C) CUDA tensors, 1 <= C <= 8, computed in fp32.
+    Returns (loss_src, loss_dst, indices1 (B,N), indices2 (B,M)); on ties the lowest index wins. The weights (float or
+    tensors broadcasting to (B,N) / (B,M)) and the reduction are applied in ATen, so tensor weights get gradients."""
+    if criterion_mode not in CD_MODES:
+        raise NotImplementedError(f'criterion_mode must be one of {CD_MODES}, got {criterion_mode!r}')
+    if reduction not in CD_REDUCTIONS:
+        raise NotImplementedError(f'reduction must be one of {CD_REDUCTIONS}, got {reduction!r}')
+    if src.dim() != 3 or dst.dim() != 3 or src.shape[0] != dst.shape[0] or src.shape[2] != dst.shape[2]:
+        raise ValueError(f'chamfer_distance takes src (B, N, C) and dst (B, M, C), got {tuple(src.shape)} and '
+                         f'{tuple(dst.shape)}')
+    if not (src.is_cuda and dst.is_cuda):
+        raise ValueError('chamfer_distance runs on CUDA tensors only (there is no CPU implementation)')
+    if not (src.is_floating_point() and dst.is_floating_point()):
+        raise ValueError('chamfer_distance takes floating-point points')
+    if src.shape[2] < 1 or src.shape[2] > 8:
+        raise ValueError(f'chamfer_distance supports 1 to 8 coordinates per point, got C={src.shape[2]}')
+    if src.numel() == 0 or dst.numel() == 0:
+        raise ValueError(f'chamfer_distance of an empty point set: src {tuple(src.shape)}, dst {tuple(dst.shape)}')
+    dist1, dist2, indices1, indices2 = _ChamferNN.apply(src, dst, criterion_mode)
+    loss_src = dist1 * src_weight
+    loss_dst = dist2 * dst_weight
+    if reduction == 'sum':
+        loss_src, loss_dst = loss_src.sum(), loss_dst.sum()
+    elif reduction == 'mean':
+        loss_src, loss_dst = loss_src.mean(), loss_dst.mean()
+    return loss_src, loss_dst, indices1, indices2
+
+
+@MODELS.register_module()
+class ChamferDistance(nn.Module):
+    """embodiedscan/models/losses/chamfer_distance.py:82-157 on the chamfer_distance kernel above."""
+
+    def __init__(self, mode='l2', reduction='mean', loss_src_weight=1.0, loss_dst_weight=1.0):
+        super().__init__()
+        _check_cd_options(mode=mode, reduction=reduction)
+        self.mode, self.reduction = mode, reduction
+        self.loss_src_weight, self.loss_dst_weight = loss_src_weight, loss_dst_weight
+
+    def forward(self, source, target, src_weight=1.0, dst_weight=1.0, reduction_override=None, return_indices=False,
+                **kwargs):
+        _check_cd_options(reduction=reduction_override)
+        reduction = reduction_override if reduction_override else self.reduction
+        loss_source, loss_target, indices1, indices2 = chamfer_distance(source, target, src_weight, dst_weight, self.mode,
+                                                                        reduction)
+        loss_source = loss_source * self.loss_src_weight
+        loss_target = loss_target * self.loss_dst_weight
+        if return_indices:
+            return loss_source, loss_target, indices1, indices2
+        return loss_source, loss_target
 
 
 @MODELS.register_module(name=['mmdet.FocalLoss', 'FocalLoss'])
@@ -127,18 +233,20 @@ class CrossEntropyLoss(nn.Module):
 
 class _BBoxCD(torch.autograd.Function):
     """Fused decode + decoupled corner-chamfer loss over the positives (csrc/head.cu::bbox_cd_loss_kernel): value and
-    the gradient w.r.t. the 12 regression channels in one launch; backward only scales the stored gradient."""
+    the gradient w.r.t. the 12 regression channels in one launch; backward only scales the stored gradient.
+    mode 'l1' / 'l2' / 'smooth_l1', group 'g8' / 'g4'; norm_decouple divides the three decoupled terms of a row by
+    clamp(|target size|, 0.1)."""
 
     @staticmethod
-    def forward(ctx, points, bbox_pred, targets, row_w, weights):
+    def forward(ctx, points, bbox_pred, targets, row_w, weights, mode='l1', group='g8', norm_decouple=False):
         P = bbox_pred.shape[0]
         dev = bbox_pred.device
         loss = torch.zeros(1, dtype=torch.float32, device=dev)
         grad = torch.empty((P, 12), dtype=torch.float32, device=dev)
         w4 = (ctypes.c_float * 4)(*[float(w) for w in weights])
         call('esb_bbox_cd_loss', ptr(points.float().contiguous()), ptr(bbox_pred.float().contiguous()),
-             ptr(targets.float().contiguous()), ptr(row_w.float().contiguous()), ctypes.cast(w4, ctypes.c_void_p), P, ptr(loss),
-             ptr(grad), stream())
+             ptr(targets.float().contiguous()), ptr(row_w.float().contiguous()), ctypes.cast(w4, ctypes.c_void_p), P,
+             _CD_MODE_CODE[mode], 8 if group == 'g8' else 4, 1 if norm_decouple else 0, ptr(loss), ptr(grad), stream())
         ctx.save_for_backward(grad)
         ctx.dtype = bbox_pred.dtype
         return loss.squeeze(0)
@@ -146,7 +254,7 @@ class _BBoxCD(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         (grad, ) = ctx.saved_tensors
-        return None, (grad * g).to(ctx.dtype), None, None, None
+        return None, (grad * g).to(ctx.dtype), None, None, None, None, None, None
 
 
 def fcaf3d_targets_batched(points: torch.Tensor, level_sizes: List[int], pt_batch: Optional[torch.Tensor],
@@ -239,6 +347,7 @@ class FCAF3DHeadRotMat(nn.Module):
         self.pts_center_threshold = pts_center_threshold
         self.center_loss = MODELS.build(center_loss)
         self.bbox_loss = MODELS.build(bbox_loss)
+        check_head_box_loss(self.bbox_loss)
         self.cls_loss = MODELS.build(cls_loss)
         self.decouple_bbox_loss = decouple_bbox_loss
         self.decouple_groups = decouple_groups
@@ -434,31 +543,37 @@ class FCAF3DHeadRotMat(nn.Module):
                                                      reduction='none')
             loss_center = (bce.squeeze(1) * w_pos).sum() * self.center_loss.loss_weight
             tgt = bbox_t[pos_inds]
-            # per-scan mean over (P_scan x 8) corners, then mean over scans -> weight 1 / (8 * P_scan * B) per corner
+            # per-scan mean over (P_scan x K) corners, then mean over scans -> weight 1 / (K * P_scan * B) per corner; K = 8
+            # for 'g8', and 4 for 'g4', whose mean is mean(corners 0-3) + mean(corners 4-7)
+            mode, group = self.bbox_loss.mode, self.bbox_loss.group
             p_scan = n_pos_local[pb_all[pos_inds]]
-            w_box = (1.0 / (8.0 * p_scan * B))[:, None]
-            fused = pos_bbox_preds.is_cuda and pos_bbox_preds.shape[1] == 12 and not self.norm_decouple_loss and \
+            w_box = (1.0 / ((8.0 if group == 'g8' else 4.0) * p_scan * B))[:, None]
+            norm = self.decouple_bbox_loss and self.norm_decouple_loss
+            fused = pos_bbox_preds.is_cuda and pos_bbox_preds.shape[1] == 12 and \
                 (not self.decouple_bbox_loss or self.decouple_groups in (3, 4))
             if fused:
                 if self.decouple_bbox_loss:
                     wts = list(self.decouple_weights[:3]) + [self.decouple_weights[3] if self.decouple_groups == 4 else 0.]
                 else:
                     wts = [0., 0., 0., 1.]
-                loss_bbox = _BBoxCD.apply(pts[pos_inds], pos_bbox_preds, tgt, w_box[:, 0] * self.bbox_loss.loss_weight, wts)
+                loss_bbox = _BBoxCD.apply(pts[pos_inds], pos_bbox_preds, tgt, w_box[:, 0] * self.bbox_loss.loss_weight, wts,
+                                          mode, group, norm)
                 return dict(loss_center=loss_center, loss_bbox=loss_bbox, loss_cls=loss_cls)
             decoded = self._bbox_pred_to_bbox(pts[pos_inds], pos_bbox_preds)
             tgt_corners = bbox_to_corners(tgt)
 
-            def cd(src):
-                return (chamfer_l1_src(bbox_to_corners(src), tgt_corners) * w_box).sum() * self.bbox_loss.loss_weight
+            def cd(src, w=w_box):
+                return (chamfer_src(bbox_to_corners(src), tgt_corners, mode, group) * w).sum() * self.bbox_loss.loss_weight
 
             if self.decouple_bbox_loss:
                 tc, ts, te = tgt[:, :3], tgt[:, 3:6], tgt[:, 6:]
                 pc, ps, pe = decoded[:, :3], decoded[:, 3:6], decoded[:, 6:]
-                assert self.decouple_groups in (3, 4) and not self.norm_decouple_loss
+                assert self.decouple_groups in (3, 4)
+                # norm_decouple_loss: the decoupled terms of a row are divided by clamp(|target size|, 0.1)
+                w_dec = w_box / ts.norm(dim=-1)[:, None].clamp(min=0.1) if norm else w_box
                 w = self.decouple_weights
-                loss_bbox = w[0] * cd(torch.cat((pc, ts, te), -1)) + w[1] * cd(torch.cat((tc, ps, te), -1)) + \
-                    w[2] * cd(torch.cat((tc, ts, pe), -1))
+                loss_bbox = w[0] * cd(torch.cat((pc, ts, te), -1), w_dec) + w[1] * cd(torch.cat((tc, ps, te), -1), w_dec) + \
+                    w[2] * cd(torch.cat((tc, ts, pe), -1), w_dec)
                 if self.decouple_groups == 4:
                     loss_bbox = loss_bbox + w[3] * cd(decoded)
             else:

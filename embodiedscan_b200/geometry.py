@@ -83,15 +83,52 @@ def box_corners_container(boxes9: torch.Tensor) -> torch.Tensor:
     return corners + boxes9[:, None, :3]
 
 
-def chamfer_l1_src(src: torch.Tensor, dst: torch.Tensor) -> torch.Tensor:
-    """(N,8,3),(N,8,3) -> (N,8) min over dst of the L1 distance (chamfer_distance.py:55-61, src->dst only)."""
-    d = (src[:, :, None, :] - dst[:, None, :, :]).abs().sum(-1)
-    return d.min(dim=2).values
+CD_MODES = ('l1', 'l2', 'smooth_l1')
+CD_GROUPS = ('g8', 'g4')
+CD_REDUCTIONS = ('mean', 'sum', 'none')
 
 
-def bbox_cd_loss(source: torch.Tensor, target: torch.Tensor, loss_weight: float = 1.0) -> torch.Tensor:
-    """BBoxCDLoss(mode='l1', group='g8', reduction='mean') (chamfer_distance.py:240-285)."""
-    return chamfer_l1_src(bbox_to_corners(source), bbox_to_corners(target)).mean() * loss_weight
+def chamfer_src(src: torch.Tensor, dst: torch.Tensor, mode: str = 'l1', group: str = 'g8') -> torch.Tensor:
+    """(N,8,3),(N,8,3) -> (N,8): per source corner, the minimum over target corners of the criterion summed over x, y, z
+    (chamfer_distance.py:55-61, src->dst only). Criteria: l1_loss, mse_loss, smooth_l1_loss (beta 1), reduction 'none'.
+    'g4' lets corners 0-3 and 4-7 search only their own half of the target corners (chamfer_distance.py:265-276)."""
+    diff = src[:, :, None, :] - dst[:, None, :, :]
+    if mode == 'l1':
+        d = diff.abs().sum(-1)
+    elif mode == 'l2':
+        d = (diff * diff).sum(-1)
+    elif mode == 'smooth_l1':
+        a = diff.abs()
+        d = torch.where(a < 1, 0.5 * a * a, a - 0.5).sum(-1)
+    else:
+        raise ValueError(f'chamfer mode must be one of {CD_MODES}, got {mode!r}')
+    if group == 'g8':
+        return d.min(dim=2).values
+    if group != 'g4':
+        raise ValueError(f'chamfer group must be one of {CD_GROUPS}, got {group!r}')
+    return torch.cat((d[:, :4, :4].min(dim=2).values, d[:, 4:, 4:].min(dim=2).values), 1)
+
+
+def bbox_cd_loss(source: torch.Tensor, target: torch.Tensor, loss_weight: float = 1.0, mode: str = 'l1',
+                 group: str = 'g8', reduction: str = 'mean', src_weight=1.0) -> torch.Tensor:
+    """BBoxCDLoss (chamfer_distance.py:240-285): boxes (N, 6/7/9); src_weight a float or a tensor broadcasting to
+    (N, 8) ('g8') or (N, 4) ('g4', applied to each half). 'g4' reduces each half on its own and adds the results, so
+    'mean' is mean(half 1) + mean(half 2) and 'none' is the (N, 4) sum of the halves."""
+    if reduction not in CD_REDUCTIONS:
+        raise ValueError(f'reduction must be one of {CD_REDUCTIONS}, got {reduction!r}')
+    d = chamfer_src(bbox_to_corners(source), bbox_to_corners(target), mode, group)
+    weighted = torch.is_tensor(src_weight) or src_weight != 1.0
+    halves = (d, ) if group == 'g8' else (d[:, :4], d[:, 4:])
+    if weighted:
+        halves = tuple(h * src_weight for h in halves)
+    if reduction == 'mean':
+        parts = [h.mean() for h in halves]
+    elif reduction == 'sum':
+        parts = [h.sum() for h in halves]
+    else:
+        parts = list(halves)
+    loss = parts[0] if len(parts) == 1 else parts[0] + parts[1]
+    return loss * loss_weight
 
 
 def box3d_overlap(corners1: torch.Tensor, corners2: torch.Tensor, eps: float = 1e-4):

@@ -29,10 +29,10 @@ import torch.nn.functional as F
 
 from . import sparse as SP
 from ._ffi import call, ptr, stream
-from .dense_heads import FCAF3DHeadRotMat
+from .dense_heads import FCAF3DHeadRotMat, check_head_box_loss
 from .detectors import SparseFeatureFusionSingleStage3DDetector, detach_log_vars, parse_losses
 from .fusion import pack_paint_metas, pack_projections, paint_points
-from .geometry import (bbox_to_corners, box3d_overlap, box_corners_container, chamfer_l1_src,
+from .geometry import (bbox_to_corners, box3d_overlap, box_corners_container, chamfer_src,
                        matrix_to_euler_angles_zxy, ortho_6d_2_mat, rotation_3d_in_euler)
 from .registry import MODELS, TASK_UTILS
 from .structures import EulerDepthInstance3DBoxes, InstanceData
@@ -421,7 +421,6 @@ class GroundingHead(nn.Module):
         self.sync_cls_avg_factor = sync_cls_avg_factor
         self.decouple_bbox_loss, self.decouple_groups = decouple_bbox_loss, decouple_groups
         self.norm_decouple_loss = norm_decouple_loss
-        assert not norm_decouple_loss, 'hot-path configuration: norm_decouple_loss=False'
         self.decouple_weights = decouple_weights or [1.0 / decouple_groups] * decouple_groups
         self.num_reg, self.box_coder = num_reg, box_coder
         assert box_coder in ('baseline', 'FCAF')
@@ -432,6 +431,7 @@ class GroundingHead(nn.Module):
         self.train_cfg, self.test_cfg = train_cfg, test_cfg
         self.loss_cls = MODELS.build(loss_cls)
         self.loss_bbox = MODELS.build(loss_bbox)
+        check_head_box_loss(self.loss_bbox)
         self.process_group = None
         self._init_layers()
         self.init_weights()
@@ -532,6 +532,44 @@ class GroundingHead(nn.Module):
                 raise NotImplementedError(type(c))
         return cost
 
+    def _box_losses(self, pred, tgt):
+        """Box loss of every decoder layer at once (grounding_head.py:758-818): pred (Ly, Npos, 9) matched predictions,
+        tgt (Npos, 9) their targets -> list of Ly scalars, each the configured BBoxCDLoss ('mean') over the pairs, with
+        the decoupled terms and norm_decouple_loss of the reference."""
+        Ly, n_pos = pred.shape[:2]
+        tgt_l = tgt[None].expand(Ly, -1, -1)
+        mode, group = self.loss_bbox.mode, self.loss_bbox.group
+
+        def pair_mean(cd, lead):
+            """(pairs, 8) per-corner distances -> mean over pairs x corners per leading index; 'g4' adds the means of
+            corners 0-3 and 4-7 (chamfer_distance.py:265-276)."""
+            if group == 'g8':
+                return cd.view(*lead, -1).mean(-1)
+            return cd.view(*lead, -1, 2, 4).mean((-3, -1)).sum(-1)
+
+        if self.decouple_bbox_loss:
+            assert self.decouple_groups in (3, 4), 'Only support groups=3 or 4 with stable performance.'
+            variants = [torch.cat((pred[..., :3], tgt_l[..., 3:]), -1),
+                        torch.cat((tgt_l[..., :3], pred[..., 3:6], tgt_l[..., 6:]), -1),
+                        torch.cat((tgt_l[..., :6], pred[..., 6:]), -1)]
+            if self.decouple_groups == 4:
+                variants.append(pred)
+            src = torch.stack(variants, 1)                                         # (Ly, Gp, Npos, 9)
+            Gp = src.shape[1]
+            cd = chamfer_src(bbox_to_corners(src.reshape(-1, 9)),
+                             bbox_to_corners(tgt_l[:, None].expand(-1, Gp, -1, -1).reshape(-1, 9)), mode, group)
+            if self.norm_decouple_loss:       # the three decoupled terms of a pair / clamp(|target size|, 0.1)
+                cd = cd.view(Ly, Gp, n_pos, 8)
+                size = tgt[:, 3:6].norm(dim=-1).clamp(min=0.1)[:, None]
+                cd = torch.cat((cd[:, :3] / size, cd[:, 3:]), 1).reshape(-1, 8)
+            per = pair_mean(cd, (Ly, Gp)) * self.loss_bbox.loss_weight             # mean over pairs x corners
+            w = per.new_tensor(self.decouple_weights[:Gp])
+            losses_bbox = list((per * w).sum(1))
+        else:
+            cd = chamfer_src(bbox_to_corners(pred.reshape(-1, 9)), bbox_to_corners(tgt_l.reshape(-1, 9)), mode, group)
+            losses_bbox = list(pair_mean(cd, (Ly, )) * self.loss_bbox.loss_weight)
+        return losses_bbox
+
     def loss(self, hidden_states, all_layers_pred_bboxes, text_feats, text_token_mask, batch_data_samples):
         cls_scores = self(hidden_states, text_feats, text_token_mask)[0].float()    # (Ly,B,nq,T)
         return self.loss_by_feat(cls_scores, all_layers_pred_bboxes, text_token_mask,
@@ -578,24 +616,7 @@ class GroundingHead(nn.Module):
         if n_pos:
             tgt = gt_boxes[bi, gi]                                                    # (Npos, 9)
             pred = pred_bboxes.float()[torch.arange(Ly, device=dev)[:, None], bi[None], qi]   # (Ly, Npos, 9)
-            tgt_l = tgt[None].expand(Ly, -1, -1)
-            if self.decouple_bbox_loss:
-                assert self.decouple_groups in (3, 4), 'Only support groups=3 or 4 with stable performance.'
-                variants = [torch.cat((pred[..., :3], tgt_l[..., 3:]), -1),
-                            torch.cat((tgt_l[..., :3], pred[..., 3:6], tgt_l[..., 6:]), -1),
-                            torch.cat((tgt_l[..., :6], pred[..., 6:]), -1)]
-                if self.decouple_groups == 4:
-                    variants.append(pred)
-                src = torch.stack(variants, 1)                                         # (Ly, Gp, Npos, 9)
-                Gp = src.shape[1]
-                cd = chamfer_l1_src(bbox_to_corners(src.reshape(-1, 9)),
-                                    bbox_to_corners(tgt_l[:, None].expand(-1, Gp, -1, -1).reshape(-1, 9)))
-                per = cd.view(Ly, Gp, -1).mean(-1) * self.loss_bbox.loss_weight        # mean over pairs x 8 corners
-                w = per.new_tensor(self.decouple_weights[:Gp])
-                losses_bbox = list((per * w).sum(1))
-            else:
-                cd = chamfer_l1_src(bbox_to_corners(pred.reshape(-1, 9)), bbox_to_corners(tgt_l.reshape(-1, 9)))
-                losses_bbox = list(cd.view(Ly, -1).mean(-1) * self.loss_bbox.loss_weight)
+            losses_bbox = self._box_losses(pred, tgt)
         else:
             losses_bbox = [pred_bboxes[l].sum() * 0 for l in range(Ly)]
         loss_dict = dict(loss_cls=losses_cls[-1], loss_bbox=losses_bbox[-1])

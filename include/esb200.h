@@ -29,6 +29,10 @@ extern "C" {
 #define ESB_ERANGE (-4)
 #define ESB_F32 0
 #define ESB_BF16 1
+/* chamfer criteria (per coordinate, summed over coordinates): |x|, x^2, smooth-L1 with beta = 1 */
+#define ESB_CD_L1 0
+#define ESB_CD_L2 1
+#define ESB_CD_SMOOTH_L1 2
 
 const char* esb_last_error(void);
 
@@ -183,9 +187,23 @@ int esb_focal_loss_bwd(const void* logits, const long long* target, long long n,
                        const float* row_w, const float* scale_dev, void* grad, int dtype, void* stream);
 
 /* box regression: _bbox_pred_to_bbox + 4 decoupled BBoxCDLoss terms (fcaf3d_head.py:1224-1281,1454-1525;
- * chamfer_distance.py:160-285) for all positives, value and gradient in one launch */
+ * chamfer_distance.py:160-285) for all positives, value and gradient in one launch.
+ * mode: ESB_CD_*; group: 8 (every source corner searches all 8 target corners) or 4 (corners 0-3 and 4-7 search their
+ * own half); norm_decouple != 0 divides the three decoupled terms of a row by clamp(|target size|, 0.1). */
 int esb_bbox_cd_loss(const float* points, const float* bbox_pred, const float* targets, const float* row_w,
-                     const float* w4_host, int P, float* loss_out, float* grad, void* stream);
+                     const float* w4_host, int P, int mode, int group, int norm_decouple, float* loss_out, float* grad,
+                     void* stream);
+
+/* ---- point-set chamfer distance (chamfer_distance.py:13-79) ---------------------------------------------------------
+ * src (B,N,C), dst (B,M,C) fp32, 1 <= C <= 8, mode ESB_CD_*. dist1 (B,N) / idx1 (B,N) int64: per source point the
+ * smallest criterion distance to dst and its index (lowest index on ties); dist2 / idx2 (B,M) the same from dst to src. */
+int esb_chamfer_fwd(const float* src, const float* dst, int B, int N, int M, int C, int mode, float* dist1,
+                    float* dist2, long long* idx1, long long* idx2, void* stream);
+/* grad_src (B,N,C) / grad_dst (B,M,C) fp32 (overwritten) from g1 = dL/d dist1 and g2 = dL/d dist2 (either may be NULL):
+ * each point's own term plus the terms of every point whose nearest neighbour it is, summed in index order. */
+int esb_chamfer_bwd(const float* src, const float* dst, const long long* idx1, const long long* idx2, const float* g1,
+                    const float* g2, int B, int N, int M, int C, int mode, float* grad_src, float* grad_dst,
+                    void* stream);
 
 /* ---- rotated BEV IoU + NMS (mmcv.ops.nms3d / nms3d_normal; fcaf3d_head.py:1666-1725) ---------------------------- */
 int esb_nms_bev_segmented(const float* boxes, const int* seg_off, int S, int max_seg, float iou_thr, int rotated,
