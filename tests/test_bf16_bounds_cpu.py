@@ -52,3 +52,145 @@ def test_selection_rules_follow_the_sm_count():
     assert B.tc_fwd_n_tile(128 * 66, 128, 132) == 64 and B.tc_fwd_n_tile(128 * 114, 256, 114) == 256
     assert B.tc_wgrad_chunk_pairs(27 * 3000, 192, 64, 132) == 512
     assert B.tc_wgrad_chunk_pairs(27 * 200000, 256, 128, 132) == 5120
+
+
+def test_dense_selection_rules():
+    assert B.conv_choose_tile(160, 120, 1, 2) == (32, 4, 1, 1)           # 128-pixel tiles that divide the output exactly
+    assert B.conv_choose_tile(3, 3, 1, 100) == (3, 3, 1, 14)             # whole 3x3 images, 14 per tile
+    assert B.conv_choose_tile(4, 4, 16, 1) == (4, 2, 16, 1)              # 3-D: TD > 1 (equal waste: the first found)
+    g = B.conv_tma_geometry(2, 1, 120, 160, 2048, 132)
+    assert g['n_tile'] == 128 and g['n_work'] == 300 * 16 and g['grid'] == 132 and not g['partial']
+    w = B.wgrad_tma_geometry(64, 1, 3, 3, 64, 64, 9, 132)
+    assert w['box'] == (4, 4, 1, 4) and w['slices'] == 5 and w['n_tiles'] == 16
+    w = B.wgrad_tma_geometry(2, 1, 60, 80, 16, 16, 9, 132)
+    assert w['per_slice'] == 8 and w['slices'] == 2 and w['last_slice_atoms'] == 1
+    assert w['n_splits'] == _cdiv(w['n_tiles'], w['tiles_per_cta']) and 0 < w['last_split'] <= w['tiles_per_cta']
+    idx = B.tile_index(2, 1, 5, 7, (4, 2, 1, 1))
+    assert idx.shape == (2, 1, 5, 7) and int(idx.max()) == 2 * 3 * 2 - 1 and int(idx[0, 0, 4, 6]) == 5
+
+
+def _cdiv(a, b):
+    return -(-a // b)
+
+
+def _emulated_conv(x, w, stride, pad, bias=None, res=None):
+    """The convolution as a bf16 kernel computes it: fp32 accumulation on the bf16 operands, one bf16 rounding."""
+    conv = torch.nn.functional.conv2d if w.dim() == 4 else torch.nn.functional.conv3d
+    y = conv(x.float(), w.float(), bias, stride, pad)
+    return (y + res.float() if res is not None else y).clamp(min=0).bfloat16()
+
+
+def test_bound_accepts_emulated_dense_conv_and_rejects_its_faults():
+    gen = torch.Generator().manual_seed(2)
+    for dims, cin, cout, k, stride, pad, S in ((2, 32, 16, 3, 1, 1, (13, 21)), (2, 16, 32, 3, 2, 1, (15, 19)),
+                                               (3, 16, 16, 3, 2, 1, (5, 7, 9))):
+        n = 3
+        x = torch.randn((n, cin) + S, generator=gen).bfloat16()
+        w = (torch.randn((cout, cin) + (k, ) * dims, generator=gen) / (cin * k ** dims) ** 0.5).bfloat16()
+        b = torch.randn(cout, generator=gen)
+        y = _emulated_conv(x, w, stride, pad, b)
+        pre, A, n_red = B.dense_conv_ref(x, w, stride, pad, b)
+        B.assert_within(y, pre.clamp(min=0), A, n_red, B.OUT_REL_BF16, 'emulated conv')
+        So = y.shape[2:]
+        tile = B.conv_choose_tile(So[-1], So[-2], So[0] if dims == 3 else 1, n)
+        faults = B.conv_fwd_faults(y, pre, x, w, stride, pad, True, tile)
+        assert len(faults) == 3
+        B.assert_rejects(faults, pre.clamp(min=0), A, n_red, B.OUT_REL_BF16)
+        # dgrad: fp32 transposed convolution of the bf16 dy, one rounding
+        dy = torch.randn(y.shape, generator=gen).bfloat16()
+        ref, A, n_red = B.dense_dgrad_ref(dy, w, x.shape, stride, pad)
+        dgrad = torch.nn.grad.conv2d_input if dims == 2 else torch.nn.grad.conv3d_input
+        dx = dgrad(x.shape, w.float(), dy.float(), stride, pad).bfloat16()
+        B.assert_within(dx, ref, A, n_red, B.OUT_REL_BF16, 'emulated dgrad')
+        tile = B.conv_choose_tile(S[-1], S[-2], S[0] if dims == 3 else 1, n)
+        B.assert_rejects(B.conv_dgrad_faults(dx, ref, dy, w, x.shape, stride, pad, tile), ref, A, n_red, B.OUT_REL_BF16)
+
+
+def test_bound_rejects_a_dropped_wgrad_split_on_integer_operands():
+    """On operands in {-1, 0, 1} the weight gradient is exact (assert_exact) and a dropped pixel split is a non-zero
+    integer in some element: the bound rejects it, although at this reduction length it could not on random operands."""
+    gen = torch.Generator().manual_seed(3)
+    n, cin, cout, S = 8, 16, 32, (30, 40)
+    geom = B.wgrad_tma_geometry(n, 1, *S, cin, cout, 9, 132)
+    assert geom['n_splits'] >= 2
+    x = B.ternary((n, cin) + S, 0.15, gen).bfloat16()
+    dy = B.ternary((n, cout) + S, 0.15, gen).bfloat16()
+    ref, A, n_red = B.dense_wgrad_ref(x, dy, (cout, cin, 3, 3), 1, 1)
+    out = torch.nn.grad.conv2d_weight(x.float(), (cout, cin, 3, 3), dy.float(), 1, 1)
+    B.assert_exact(out, ref, A, 'emulated wgrad', out_bf16=False)
+    faults = B.wgrad_split_faults(out, x, dy, (cout, cin, 3, 3), 1, 1, geom)
+    B.assert_rejects(faults, ref, A, n_red, B.OUT_REL_F32)
+
+
+def _emulated_attention(q, k, v, pad, scale, do):
+    """Attention as csrc/attn_tc.cu computes it, in fp32: P rounded to bf16 before P V and P^T dO (l from the unrounded
+    p), O stored bf16 and read back for delta, dS^T rounded to bf16 for dK and dQ."""
+    qf, kf, vf, dof = q.float(), k.float(), v.float(), do.float()
+    s = scale * qf @ kf.transpose(-1, -2)
+    s = s.masked_fill(pad[:, None, None, :], -float('inf'))
+    m = s.amax(-1, keepdim=True)
+    m = torch.where(torch.isfinite(m), m, torch.zeros_like(m))
+    p = torch.exp(s - m)
+    l = p.sum(-1, keepdim=True)
+    inv = torch.where(l > 0, 1 / l, torch.zeros_like(l))
+    o = ((p.bfloat16().float() @ vf) * inv).bfloat16()
+    P = p * inv
+    delta = (o.float() * dof).sum(-1, keepdim=True)
+    dS = (P * (dof @ vf.transpose(-1, -2) - delta) * scale).bfloat16().float()
+    dv = (P.bfloat16().float().transpose(-1, -2) @ dof).bfloat16()
+    dk = (dS.transpose(-1, -2) @ qf).bfloat16()
+    dq = dS @ kf
+    return o, dq, dk, dv
+
+
+def test_bound_accepts_emulated_attention_and_rejects_its_faults():
+    gen = torch.Generator().manual_seed(4)
+    Bn, H, Lq, Lk = 3, 2, 70, 300
+    q, k, v, do = (torch.randn(Bn, H, L, 32, generator=gen).bfloat16() for L in (Lq, Lk, Lk, Lq))
+    pad = torch.zeros(Bn, Lk, dtype=torch.bool)
+    pad[0, 250:] = True
+    pad[1, :40] = True
+    pad[2] = True
+    k[:, :, :40] *= 16                                  # padded keys with large values: a leak must be visible
+    v[:, :, :40] = 1000.0
+    scale = 32 ** -0.5
+    ref = B.attn_ref(q, k, v, pad, scale, do)
+    outs = dict(zip(('o', 'dq', 'dk', 'dv'), _emulated_attention(q, k, v, pad, scale, do)))
+    for nm, out in outs.items():
+        val, A, fixed = ref[nm]
+        B.assert_within(out, val, A, 1, B.OUT_REL_F32 if nm == 'dq' else B.OUT_REL_BF16, f'emulated attention {nm}',
+                        fixed=fixed)
+        assert bool((out[2] == 0).all()), 'a scan without live keys must give exact zeros'
+    assert bool((ref['lse'][2] == -float('inf')).all())
+    val, A, fixed = ref['o']
+    faults = B.attn_fwd_faults(outs['o'], q, k, v, pad, scale)
+    assert len(faults) == 2
+    B.assert_rejects(faults, val, A, 1, B.OUT_REL_BF16, fixed)
+    val, A, fixed = ref['dq']
+    B.assert_rejects(B.attn_dq_faults(outs['dq'], k, ref['dS']), val, A, 1, B.OUT_REL_F32, fixed)
+
+
+def test_bound_accepts_emulated_painting_and_rejects_its_faults():
+    """Painting as csrc/paint.cu computes it (fp32 sums of bf16 features, one bf16 rounding forward; fp32 backward) passes
+    the bound of bf16_bounds.paint_ref, and each fault of paint_faults is rejected."""
+    gen = torch.Generator().manual_seed(5)
+    Bn, V, Hf, Wf, N, C = 2, 9, 12, 16, 400, 40
+    tx = torch.randint(-3, 4, (Bn, V), generator=gen).double() + 0.125
+    ty = torch.randint(-3, 4, (Bn, V), generator=gen).double() - 0.375
+    front = torch.rand(Bn, V, generator=gen) > 0.2
+    batch = torch.randint(0, Bn, (N, ), generator=gen)
+    pts = torch.stack([torch.randint(-20, 4 * (Wf + 5), (N, ), generator=gen), torch.randint(-20, 4 * (Hf + 5), (N, ),
+                      generator=gen), torch.zeros(N, dtype=torch.long)], 1).double() * 0.25
+    feat = torch.randn(Bn * V, Hf, Wf, C, generator=gen).bfloat16()
+    dout = torch.randn(N, C, generator=gen).bfloat16()
+    pad = (Hf - 1.0, Wf - 1.0)
+    ref = B.paint_ref(feat, pts, batch, tx, ty, front, pad, dout)
+    emu = B.paint_ref(feat, pts, batch, tx, ty, front, pad, dout, dtype=torch.float32)
+    assert bool((ref['hit'] & ~ref['valid']).any())
+    out, dfeat = emu['fwd'][0].bfloat16(), emu['bwd'][0]
+    B.assert_within(out, *ref['fwd'], B.OUT_REL_BF16, 'emulated paint fwd', c=B.C_PAINT)
+    B.assert_within(dfeat, *ref['bwd'], B.OUT_REL_F32, 'emulated paint bwd', c=B.C_PAINT)
+    fwd_f, bwd_f = B.paint_faults(out, dfeat, ref, feat, dout)
+    assert len(fwd_f) == 3 and len(bwd_f) == 2
+    B.assert_rejects(fwd_f, *ref['fwd'], B.OUT_REL_BF16, c=B.C_PAINT)
+    B.assert_rejects(bwd_f, *ref['bwd'], B.OUT_REL_F32, c=B.C_PAINT)
