@@ -67,6 +67,8 @@ SIGNATURES = {
     'esb_nms_bev_segmented': ('ppiifipp', 'i'),
     'esb_iou_bev_pairwise': ('pipiipp', 'i'),
     'esb_box3d_overlap': ('pipippp', 'i'),
+    'esb_nms3d_9dof_workspace_bytes': ('iii', 'z'),
+    'esb_nms3d_9dof': ('pppp' + 'ii' + 'ff' + 'ii' + 'ppp' + 'zp', 'i'),
     'esb_hungarian_batch': ('ppiiippp', 'i'),
     'esb_img_normalize': ('piiiiippiipip', 'i'),
     'esb_unproject_depth_workspace_bytes': ('iii', 'z'),
@@ -87,7 +89,7 @@ KERNELS_PER_CALL = {
     'esb_focal_loss_fwd': 1, 'esb_focal_loss_bwd': 1, 'esb_nms_bev_segmented': 1, 'esb_iou_bev_pairwise': 1,
     'esb_img_normalize': 1, 'esb_unproject_depth': 3, 'esb_grad_clip_coef': 2, 'esb_adamw_step': 1,
     'esb_cast_f32_to_bf16': 1, 'esb_spconv_tc_fwd': 1, 'esb_spconv_tc_wgrad': 1, 'esb_kmap_tile_masks': 1,
-    'esb_chamfer_fwd': 2, 'esb_chamfer_bwd': 4,
+    'esb_chamfer_fwd': 2, 'esb_chamfer_bwd': 4, 'esb_nms3d_9dof': 2,
 }
 launch_counter = {'kernels': 0, 'calls': 0, 'by_name': {}}
 

@@ -142,3 +142,52 @@ def box3d_overlap(corners1: torch.Tensor, corners2: torch.Tensor, eps: float = 1
     iou = torch.empty((n1, n2), dtype=torch.float32, device=c1.device)
     call('esb_box3d_overlap', ptr(c1), n1, ptr(c2), n2, ptr(vol), ptr(iou), stream())
     return vol, iou
+
+
+def nms3d_9dof(boxes9: torch.Tensor, scores: torch.Tensor, labels: torch.Tensor, iou_thr: float,
+               score_thr: float = float('-inf'), topk_per_class=None, seg_off=None, num_classes=None):
+    """Class-agnostic greedy NMS on the exact 9-DoF 3D IoU with a score threshold and a per-label cap, the semantics of
+    the reference's ``nms_filter`` (demo/demo.py:107-130): walking the boxes by descending score (stable: ties keep
+    input order), a box is skipped when its label already has `topk_per_class` kept boxes, when its score is below
+    `score_thr`, or when its IoU with a kept box exceeds `iou_thr`; a skipped box suppresses nothing.
+
+    boxes9 (M,9), scores (M), labels (M) CUDA tensors -> LongTensor of kept input indices in selection order. With
+    `seg_off` (S+1 host integers, segment s = rows seg_off[s]:seg_off[s+1]) every segment is filtered on its own in
+    the same launch and a list of S index tensors comes back. Runs in libesb200.so (csrc/nms3d.cu, no CPU fallback);
+    the kept counts of all segments are read back once. `num_classes` bounds the labels when the cap is set; left
+    None it is read from ``labels.max()`` (one more small read-back)."""
+    from ._ffi import call, ptr, query, stream
+    assert boxes9.is_cuda, 'nms3d_9dof runs in libesb200.so (no CPU fallback)'
+    assert boxes9.dim() == 2 and boxes9.shape[1] == 9 and scores.shape == labels.shape == boxes9.shape[:1]
+    assert iou_thr >= 0, 'iou_thr must be >= 0'
+    dev, M = boxes9.device, boxes9.shape[0]
+    offs = [0, M] if seg_off is None else [int(o) for o in seg_off]
+    assert offs[0] == 0 and offs[-1] == M and all(a <= b for a, b in zip(offs, offs[1:])), 'seg_off must cover 0..M'
+    S = len(offs) - 1
+    lens = [b - a for a, b in zip(offs, offs[1:])]
+    max_seg = max(lens) if lens else 0
+    if M == 0:
+        out = [torch.empty(0, dtype=torch.long, device=dev) for _ in range(S)]
+        return out[0] if seg_off is None else out
+    scores = scores.float()
+    order = torch.sort(scores, stable=True, descending=True).indices
+    if S > 1:                                     # segment-major, score-descending inside each segment, still stable
+        seg_of = torch.repeat_interleave(torch.arange(S, device=dev), torch.tensor(lens, device=dev), output_size=M)
+        order = order[torch.sort(seg_of[order], stable=True).indices]
+    if topk_per_class is None:                    # no cap: one label, a limit no count reaches
+        lab, topk, ncls = torch.zeros(M, dtype=torch.int32, device=dev), 2 ** 31 - 1, 1
+    else:
+        lab, topk = labels[order].to(torch.int32).contiguous(), int(topk_per_class)
+        ncls = int(num_classes) if num_classes is not None else int(labels.max()) + 1
+    b = boxes9.float()[order].contiguous()
+    sc = scores[order].contiguous()
+    so = torch.tensor(offs, dtype=torch.int32).to(dev)
+    keep = torch.empty(M, dtype=torch.int32, device=dev)
+    n_keep = torch.empty(S, dtype=torch.int32, device=dev)
+    wsb = query('esb_nms3d_9dof_workspace_bytes', M, S, max_seg)
+    ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+    call('esb_nms3d_9dof', ptr(b), ptr(sc), ptr(lab), ptr(so), S, max_seg, float(iou_thr), float(score_thr), topk,
+         max(ncls, 1), ptr(keep), ptr(n_keep), ptr(ws), wsb, stream())
+    counts = n_keep.tolist()
+    out = [order[keep[o:o + k].long()] for o, k in zip(offs, counts)]
+    return out[0] if seg_off is None else out

@@ -214,6 +214,20 @@ int esb_iou_bev_pairwise(const float* a, int na, const float* b, int nb, int rot
 int esb_box3d_overlap(const float* corners1, int n1, const float* corners2, int n2, float* vol, float* iou,
                       void* stream);
 
+/* ---- greedy NMS on the exact 9-DoF 3D IoU (the demo's final box filter `nms_filter`, demo/demo.py:84-130), batched over
+ * S segments. boxes9 (M,9) = centre, size, ZXY Euler angles; scores (M); labels (M) in [0, num_classes); seg_off (S+1).
+ * Candidates are already score-descending inside each segment. Walking a segment in order, a candidate is skipped when
+ * its label already has topk_per_class kept boxes, when score < score_thr, or when its IoU with a kept box exceeds
+ * iou_thr (>= 0); skipped candidates suppress nothing. Segment s writes the kept positions (indices into the M rows) to
+ * keep[seg_off[s] ..) in selection order and their count to n_keep[s]. A box with a size <= 0 or a non-finite value has
+ * IoU 0 with every box: it can be kept, never suppresses and is never suppressed. A label outside [0, num_classes) is
+ * never kept. After the call the first 3*S unsigned long long of ws hold, per segment, the pairs tested, the pairs
+ * left by the bounding-sphere test and the pairs left by the separating-axis test (those ran the exact clipping). */
+size_t esb_nms3d_9dof_workspace_bytes(int M, int S, int max_seg);
+int esb_nms3d_9dof(const float* boxes9, const float* scores, const int* labels, const int* seg_off, int S, int max_seg,
+                   float iou_thr, float score_thr, int topk_per_class, int num_classes, int* keep, int* n_keep, void* ws,
+                   size_t ws_bytes, void* stream);
+
 /* ---- batched one-to-one assignment (HungarianAssigner3D.assign: hungarian_assigner.py:110-126 -> scipy
  * linear_sum_assignment on the host, 7 layers x batch times per iteration from grounding_head.py:398).
  * cost: (n_problems, n_pred, ld_gt) fp32, problem p uses columns [0, n_gt[p]); n_gt[p] <= ld_gt <= n_pred.
