@@ -330,8 +330,77 @@ def multiclass_nms_bev(bboxes: torch.Tensor, scores: torch.Tensor, score_thr: fl
     return out_boxes, s_s[sel], cls_s[sel]
 
 
+class SparseFPN(nn.Module):
+    """The pruned sparse FPN of FCAF3D (fcaf3d_head.py:993-1114, mink_neck.py:133-244), shared by ``FCAF3DHeadRotMat``
+    and ``MinkNeck``. Subclasses set ``pts_prune_threshold`` and call ``_init_fpn`` where the reference builds the
+    blocks, so parameters register in the reference's order."""
+
+    def _init_fpn(self, in_channels, out_channels):
+        self.pruning = SP.MinkowskiPruning()
+        for i in range(len(in_channels)):
+            if i > 0:
+                setattr(self, f'up_block_{i}', self._make_up_block(in_channels[i], in_channels[i - 1]))
+            setattr(self, f'out_block_{i}', self._make_block(in_channels[i], out_channels))
+
+    @staticmethod
+    def _make_block(in_channels, out_channels):
+        return nn.Sequential(SP.MinkowskiConvolution(in_channels, out_channels, kernel_size=3, dimension=3),
+                             SP.MinkowskiBatchNorm(out_channels), SP.MinkowskiELU())
+
+    @staticmethod
+    def _make_up_block(in_channels, out_channels):
+        return nn.Sequential(
+            SP.MinkowskiGenerativeConvolutionTranspose(in_channels, out_channels, kernel_size=2, stride=2, dimension=3),
+            SP.MinkowskiBatchNorm(out_channels), SP.MinkowskiELU(),
+            SP.MinkowskiConvolution(out_channels, out_channels, kernel_size=3, dimension=3),
+            SP.MinkowskiBatchNorm(out_channels), SP.MinkowskiELU())
+
+    def _run_block(self, seq: nn.Sequential, x: SP.SparseTensor) -> SP.SparseTensor:
+        """(conv|deconv) -> BN -> ELU triples with BN+ELU fused into one kernel."""
+        mods = list(seq)
+        assert len(mods) % 3 == 0
+        for i in range(0, len(mods), 3):
+            x = SP.conv_norm_act(mods[i], mods[i + 1], SP.ACT_ELU, x, training=self.training)
+        return x
+
+    def _top_down(self, inputs: List[SP.SparseTensor], level_fn) -> list:
+        """Top-down pass (fcaf3d_head.py:993-1020): from the coarsest level, up block, union add with the finer input and
+        prune by the coarser level's score, then the level's out block. ``level_fn(i, out)`` returns (result, prune score
+        for the next finer level); the results come back coarse -> fine."""
+        results = []
+        x = inputs[-1]
+        prune_score = None
+        for i in range(len(inputs) - 1, -1, -1):
+            if i < len(inputs) - 1:
+                x = self._run_block(getattr(self, f'up_block_{i + 1}'), x)
+                x = inputs[i] + x
+                x = self._prune(x, prune_score)
+            res, prune_score = level_fn(i, self._run_block(getattr(self, f'out_block_{i}'), x))
+            results.append(res)
+        return results
+
+    def _prune(self, x: SP.SparseTensor, scores: SP.SparseTensor) -> SP.SparseTensor:
+        """Per-scan top-k by the multilinearly interpolated parent max-class score (fcaf3d_head.py:1091-1114).
+        Identity whenever every scan holds <= pts_prune_threshold rows."""
+        if len(x) <= self.pts_prune_threshold:      # no scan can exceed the threshold: skip without a host sync
+            return x
+        perms, _, counts = x.cmap.decomposition(x.coordinate_manager.batch_size)
+        if max(counts) <= self.pts_prune_threshold:
+            return x
+        with torch.no_grad():
+            interpolated = scores.features_at_coordinates(x.C)      # integer child coordinates: the fused kernel
+            prune_mask = torch.zeros(len(interpolated), dtype=torch.bool, device=x.device)
+            for perm in perms:
+                score = interpolated[perm].squeeze(1)
+                topk = min(len(score), self.pts_prune_threshold)
+                # torch.topk leaves ties unspecified; frozen rule: descending score, lowest row first among ties
+                ids = torch.sort(score, descending=True, stable=True).indices[:topk]
+                prune_mask[perm[ids]] = True
+        return self.pruning(x, prune_mask)
+
+
 @MODELS.register_module()
-class FCAF3DHeadRotMat(nn.Module):
+class FCAF3DHeadRotMat(SparseFPN):
 
     def __init__(self, num_classes: int, in_channels: Tuple[int], out_channels: int, num_reg_outs: int,
                  voxel_size: float, pts_prune_threshold: int, pts_assign_threshold: int, pts_center_threshold: int,
@@ -359,25 +428,8 @@ class FCAF3DHeadRotMat(nn.Module):
         self.init_weights()
         self.process_group = None
 
-    @staticmethod
-    def _make_block(in_channels, out_channels):
-        return nn.Sequential(SP.MinkowskiConvolution(in_channels, out_channels, kernel_size=3, dimension=3),
-                             SP.MinkowskiBatchNorm(out_channels), SP.MinkowskiELU())
-
-    @staticmethod
-    def _make_up_block(in_channels, out_channels):
-        return nn.Sequential(
-            SP.MinkowskiGenerativeConvolutionTranspose(in_channels, out_channels, kernel_size=2, stride=2, dimension=3),
-            SP.MinkowskiBatchNorm(out_channels), SP.MinkowskiELU(),
-            SP.MinkowskiConvolution(out_channels, out_channels, kernel_size=3, dimension=3),
-            SP.MinkowskiBatchNorm(out_channels), SP.MinkowskiELU())
-
     def _init_layers(self, in_channels, out_channels, num_reg_outs, num_classes):
-        self.pruning = SP.MinkowskiPruning()
-        for i in range(len(in_channels)):
-            if i > 0:
-                setattr(self, f'up_block_{i}', self._make_up_block(in_channels[i], in_channels[i - 1]))
-            setattr(self, f'out_block_{i}', self._make_block(in_channels[i], out_channels))
+        self._init_fpn(in_channels, out_channels)
         self.conv_center = SP.MinkowskiConvolution(out_channels, 1, kernel_size=1, dimension=3)
         self.conv_reg = SP.MinkowskiConvolution(out_channels, num_reg_outs, kernel_size=1, dimension=3)
         self.conv_cls = SP.MinkowskiConvolution(out_channels, num_classes, kernel_size=1, bias=True, dimension=3)
@@ -390,32 +442,13 @@ class FCAF3DHeadRotMat(nn.Module):
         nn.init.constant_(self.conv_cls.bias, -4.59511985013459)  # bias_init_with_prob(.01)
 
     # ---- forward ------------------------------------------------------------------------------------------
-    def _run_block(self, seq: nn.Sequential, x: SP.SparseTensor) -> SP.SparseTensor:
-        """(conv|deconv) -> BN -> ELU triples with BN+ELU fused into one kernel."""
-        mods = list(seq)
-        assert len(mods) % 3 == 0
-        for i in range(0, len(mods), 3):
-            x = SP.conv_norm_act(mods[i], mods[i + 1], SP.ACT_ELU, x, training=self.training)
-        return x
-
     def _forward_levels(self, x: List[SP.SparseTensor]):
         """Top-down pass (fcaf3d_head.py:993-1020). Returns, per level (fine -> coarse), a dict of whole-batch tensors
         center (N,1), bbox (N,12), cls (N,C), points (N,3), batch (N,) int32, perms (per-scan row indices)."""
-        outs = []
-        inputs = x
-        x = inputs[-1]
-        prune_score = None
-        f0 = inputs[-1].F
+        f0 = x[-1].F
         w_all = self._head_weights(f0) if f0.is_cuda and f0.dtype == torch.bfloat16 else None
-        for i in range(len(inputs) - 1, -1, -1):
-            if i < len(inputs) - 1:
-                x = self._run_block(getattr(self, f'up_block_{i + 1}'), x)
-                x = inputs[i] + x
-                x = self._prune(x, prune_score)
-            out = self._run_block(getattr(self, f'out_block_{i}'), x)
-            lv, prune_score = self._forward_single_level(out, self.scales[i], need_prune_score=i > 0, w_all=w_all)
-            outs.append(lv)
-        return outs[::-1]
+        return self._top_down(x, lambda i, out: self._forward_single_level(out, self.scales[i], need_prune_score=i > 0,
+                                                                           w_all=w_all))[::-1]
 
     def forward(self, x: List[SP.SparseTensor]):
         """Reference return format: four lists (level-major) of per-scan tensor lists."""
@@ -427,25 +460,6 @@ class FCAF3DHeadRotMat(nn.Module):
             cls_preds.append([lv['cls'][p] for p in perms])
             points.append([lv['points'][p] for p in perms])
         return center_preds, bbox_preds, cls_preds, points
-
-    def _prune(self, x: SP.SparseTensor, scores: SP.SparseTensor) -> SP.SparseTensor:
-        """Per-scan top-k by the multilinearly interpolated parent max-class score (fcaf3d_head.py:1091-1114).
-        Identity whenever every scan holds <= pts_prune_threshold rows."""
-        if len(x) <= self.pts_prune_threshold:      # no scan can exceed the threshold: skip without a host sync
-            return x
-        perms, _, counts = x.cmap.decomposition(x.coordinate_manager.batch_size)
-        if max(counts) <= self.pts_prune_threshold:
-            return x
-        with torch.no_grad():
-            interpolated = scores.features_at_coordinates(x.C)      # integer child coordinates: the fused kernel
-            prune_mask = torch.zeros(len(interpolated), dtype=torch.bool, device=x.device)
-            for perm in perms:
-                score = interpolated[perm].squeeze(1)
-                topk = min(len(score), self.pts_prune_threshold)
-                # torch.topk leaves ties unspecified; frozen rule: descending score, lowest row first among ties
-                ids = torch.sort(score, descending=True, stable=True).indices[:topk]
-                prune_mask[perm[ids]] = True
-        return self.pruning(x, prune_mask)
 
     def _head_weights(self, f: torch.Tensor):
         """[cls | centre | reg | zero pad] (C_in, width) fp32, width a multiple of 64: the operand of the ONE tensor-core GEMM

@@ -2,7 +2,8 @@
 (embodiedscan/models/detectors/sparse_featfusion_single_stage.py:28-426,
 embodiedscan/models/data_preprocessors/data_preprocessor.py:23-339) — same constructor arguments and
 ``forward(inputs, data_samples, mode)`` contract, so mmengine's ``train_step / val_step / test_step`` (mirrored
-here for the mmengine-less image) drive it unchanged.
+here for the mmengine-less image) drive it unchanged. ``MultiModal3DModel`` holds that contract and the input front half
+for the detector, occupancy and grounding models alike.
 """
 from typing import Dict, List, Optional, Union
 
@@ -15,6 +16,7 @@ from . import _ffi
 from . import sparse as SP
 from ._ffi import call, ptr, stream
 from .fusion import pack_paint_metas, pack_projections, paint_points
+from .precision import fence_losses, fp32_exact
 from .registry import MODELS
 from .structures import Det3DDataSample, InstanceData
 
@@ -126,34 +128,57 @@ class Det3DDataPreprocessor(nn.Module):
         return {'inputs': out, 'data_samples': data_samples}
 
 
-@MODELS.register_module()
-class SparseFeatureFusionSingleStage3DDetector(nn.Module):
+def preprocessor_cfg(data_preprocessor: Optional[dict], compute_dtype) -> Optional[dict]:
+    """A model's preprocessor config: a copy that writes images in the model's compute dtype, ``Det3DDataPreprocessor``
+    unless the config names another type."""
+    if isinstance(data_preprocessor, dict):
+        data_preprocessor = dict(data_preprocessor, compute_dtype=compute_dtype)
+        data_preprocessor.setdefault('type', 'Det3DDataPreprocessor')
+    return data_preprocessor
 
-    def __init__(self, backbone, backbone_3d, bbox_head, neck=None, neck_3d=None, coord_type: str = 'CAMERA',
-                 train_cfg: Optional[dict] = None, test_cfg: Optional[dict] = None,
-                 data_preprocessor: Optional[dict] = None, use_xyz_feat: bool = False, init_cfg: Optional[dict] = None,
-                 compute_dtype=torch.float32):
-        super().__init__()
-        assert neck is None and neck_3d is None, 'no configured hot-path model uses neck / neck_3d here'
-        self.compute_dtype = compute_dtype
-        if isinstance(data_preprocessor, dict):
-            data_preprocessor = dict(data_preprocessor, compute_dtype=compute_dtype)
-            data_preprocessor.setdefault('type', 'Det3DDataPreprocessor')
-        self.data_preprocessor = MODELS.build(data_preprocessor) if data_preprocessor is not None else None
-        self.backbone = MODELS.build(backbone)
-        self.backbone_3d = MODELS.build(backbone_3d)
-        bbox_head = dict(bbox_head)
-        bbox_head.update(train_cfg=train_cfg)
-        bbox_head.update(test_cfg=test_cfg)
-        self.bbox_head = MODELS.build(bbox_head)
-        self.coord_type = coord_type
-        self.train_cfg, self.test_cfg = train_cfg, test_cfg
-        self.voxel_size = bbox_head['voxel_size']
-        self.use_xyz_feat = use_xyz_feat
-        self.overlap_2d_3d = True
-        self._side_stream = None
 
-    # ---- feature extraction (sparse_featfusion_single_stage.py:86-221) --------------------------------------
+class MultiModal3DModel(nn.Module):
+    """What the detector, occupancy and grounding models share: mmengine's ``BaseModel`` contract (``forward(mode=...)``,
+    ``train_step / val_step / test_step``), the multi-view image batch, and the sparse front half of the detector and the
+    grounder (voxelise -> MinkResNet -> paint every level from the scan's views). Subclasses set ``compute_dtype`` and
+    ``data_preprocessor`` and implement ``loss`` / ``predict``."""
+
+    def forward(self, inputs: Union[dict, List[dict]], data_samples=None, mode: str = 'tensor', **kwargs):
+        if self.compute_dtype == torch.float32:
+            # fp32 = the parity arithmetic: library contractions stay out of TF32 in forward AND backward
+            with fp32_exact():
+                return fence_losses(self._forward(inputs, data_samples, mode, **kwargs))
+        return self._forward(inputs, data_samples, mode, **kwargs)
+
+    def _forward(self, inputs, data_samples, mode, **kwargs):
+        if mode == 'loss':
+            return self.loss(inputs, data_samples, **kwargs)
+        if mode == 'predict':
+            return self.predict(inputs, data_samples, **kwargs)
+        raise RuntimeError(f'Invalid mode "{mode}". Only supports loss and predict mode')
+
+    # ---- mmengine BaseModel contract (†upstream) -------------------------------------------------------------
+    def train_step(self, data, optim_wrapper):
+        data = self.data_preprocessor(data, True)
+        loss, log_vars = parse_losses(self(**data, mode='loss'))
+        optim_wrapper.update_params(loss)
+        return detach_log_vars(log_vars)
+
+    @torch.no_grad()
+    def val_step(self, data):
+        data = self.data_preprocessor(data, False)
+        return self(**data, mode='predict')
+
+    test_step = val_step
+
+    # ---- shared feature extraction (sparse_featfusion_single_stage.py:86-221) --------------------------------
+    def view_batch(self, img: torch.Tensor) -> torch.Tensor:
+        """(B, V, 3, H, W) images -> the (B*V, 3, H, W) batch of the 2D backbone, channels-last, in the compute dtype."""
+        img4 = img.reshape([-1] + list(img.shape)[2:]).to(self.compute_dtype)
+        if not img4.is_contiguous(memory_format=torch.channels_last):
+            img4 = img4.contiguous(memory_format=torch.channels_last)
+        return img4
+
     def voxelize(self, points: List[torch.Tensor]):
         dev = points[0].device
         n_tot = sum(p.shape[0] for p in points)
@@ -168,15 +193,53 @@ class SparseFeatureFusionSingleStage3DDetector(nn.Module):
             feats.append(p if self.use_xyz_feat else p[:, 3:])
         return coords, torch.cat(feats)
 
+    def sparse_levels(self, points: List[torch.Tensor]) -> List[SP.SparseTensor]:
+        """Voxelise the point clouds (one sample each) and run the sparse 3D backbone: its levels, fine -> coarse."""
+        coordinates, features = self.voxelize(points)
+        x = SP.SparseTensor(coordinates=coordinates, features=features.to(self.compute_dtype), batch_size=len(points))
+        return self.backbone_3d(x)
+
+    def paint_levels(self, x: List[SP.SparseTensor], img_features, img: torch.Tensor, batch_img_metas) -> None:
+        """Append to every level's features the image features its voxels project onto, over all V views of each scan."""
+        dev = img.device
+        metas = pack_paint_metas(batch_img_metas, dev)
+        proj = pack_projections(batch_img_metas, self.coord_type, dev)
+        pad_hw = tuple(img.shape[-2:])
+        for level_idx in range(len(x)):
+            painted = paint_points(img_features[level_idx], x[level_idx].C, metas, proj, self.voxel_size, pad_hw,
+                                   img.shape[1])
+            x[level_idx] = x[level_idx].replace_feature(torch.cat([x[level_idx].F, painted.to(x[level_idx].F.dtype)], 1))
+
+
+@MODELS.register_module()
+class SparseFeatureFusionSingleStage3DDetector(MultiModal3DModel):
+
+    def __init__(self, backbone, backbone_3d, bbox_head, neck=None, neck_3d=None, coord_type: str = 'CAMERA',
+                 train_cfg: Optional[dict] = None, test_cfg: Optional[dict] = None,
+                 data_preprocessor: Optional[dict] = None, use_xyz_feat: bool = False, init_cfg: Optional[dict] = None,
+                 compute_dtype=torch.float32):
+        super().__init__()
+        assert neck is None and neck_3d is None, 'no configured hot-path model uses neck / neck_3d here'
+        self.compute_dtype = compute_dtype
+        data_preprocessor = preprocessor_cfg(data_preprocessor, compute_dtype)
+        self.data_preprocessor = MODELS.build(data_preprocessor) if data_preprocessor is not None else None
+        self.backbone = MODELS.build(backbone)
+        self.backbone_3d = MODELS.build(backbone_3d)
+        bbox_head = dict(bbox_head)
+        bbox_head.update(train_cfg=train_cfg)
+        bbox_head.update(test_cfg=test_cfg)
+        self.bbox_head = MODELS.build(bbox_head)
+        self.coord_type = coord_type
+        self.train_cfg, self.test_cfg = train_cfg, test_cfg
+        self.voxel_size = bbox_head['voxel_size']
+        self.use_xyz_feat = use_xyz_feat
+        self.overlap_2d_3d = True
+        self._side_stream = None
+
     def extract_feat(self, batch_inputs_dict: Dict[str, torch.Tensor], batch_data_samples) -> List[SP.SparseTensor]:
-        points = batch_inputs_dict['points']
         img = batch_inputs_dict['imgs']
-        batch_img_metas = [ds.metainfo for ds in batch_data_samples]
         assert img.dim() == 5, 'multi-view input (B, n_views, C, H, W)'
-        B, V = img.shape[:2]
-        img4 = img.reshape([-1] + list(img.shape)[2:]).to(self.compute_dtype)
-        if not img4.is_contiguous(memory_format=torch.channels_last):
-            img4 = img4.contiguous(memory_format=torch.channels_last)
+        img4 = self.view_batch(img)
 
         # Two streams: the dense per-view 2D backbone runs on a side stream while the main stream builds the coordinate
         # plan (whose row-count read-backs synchronise only the main stream) and runs the sparse 3D backbone; they
@@ -195,22 +258,12 @@ class SparseFeatureFusionSingleStage3DDetector(nn.Module):
         else:
             img_features = self.backbone(img4)
 
-        coordinates, features = self.voxelize(points)
-        x = SP.SparseTensor(coordinates=coordinates, features=features.to(self.compute_dtype), batch_size=len(points))
-        x = self.backbone_3d(x)
-        num_levels = len(x)
+        x = self.sparse_levels(batch_inputs_dict['points'])
         if side is not None:
             main.wait_stream(side)
             for f in img_features:
                 f.record_stream(main)
-
-        dev = img.device
-        metas = pack_paint_metas(batch_img_metas, dev)
-        proj = pack_projections(batch_img_metas, self.coord_type, dev)
-        pad_hw = tuple(img.shape[-2:])
-        for level_idx in range(num_levels):
-            painted = paint_points(img_features[level_idx], x[level_idx].C, metas, proj, self.voxel_size, pad_hw, V)
-            x[level_idx] = x[level_idx].replace_feature(torch.cat([x[level_idx].F, painted.to(x[level_idx].F.dtype)], 1))
+        self.paint_levels(x, img_features, img, [ds.metainfo for ds in batch_data_samples])
         return x
 
     def loss(self, batch_inputs_dict, batch_data_samples, **kwargs):
@@ -221,18 +274,6 @@ class SparseFeatureFusionSingleStage3DDetector(nn.Module):
         x = self.extract_feat(batch_inputs_dict, batch_data_samples)
         results_list = self.bbox_head.predict(x, batch_data_samples, **kwargs)
         return self.add_pred_to_datasample(batch_data_samples, results_list)
-
-    def forward(self, inputs: Union[dict, List[dict]], data_samples=None, mode: str = 'tensor', **kwargs):
-        if mode == 'loss':
-            if self.compute_dtype == torch.float32:
-                # fp32 = the parity arithmetic: library convolutions stay out of TF32 in forward AND backward
-                from .precision import fence_losses, fp32_exact
-                with fp32_exact():
-                    return fence_losses(self.loss(inputs, data_samples, **kwargs))
-            return self.loss(inputs, data_samples, **kwargs)
-        if mode == 'predict':
-            return self.predict(inputs, data_samples, **kwargs)
-        raise RuntimeError(f'Invalid mode "{mode}". Only supports loss and predict mode')
 
     @staticmethod
     def add_pred_to_datasample(data_samples, data_instances_3d=None, data_instances_2d=None):
@@ -245,21 +286,6 @@ class SparseFeatureFusionSingleStage3DDetector(nn.Module):
             ds.pred_instances_3d = data_instances_3d[i]
             ds.pred_instances = data_instances_2d[i]
         return data_samples
-
-    # ---- mmengine BaseModel contract (†upstream) -------------------------------------------------------------
-    def train_step(self, data, optim_wrapper):
-        data = self.data_preprocessor(data, True)
-        losses = self(**data, mode='loss')
-        loss, log_vars = parse_losses(losses)
-        optim_wrapper.update_params(loss)
-        return detach_log_vars(log_vars)
-
-    @torch.no_grad()
-    def val_step(self, data):
-        data = self.data_preprocessor(data, False)
-        return self(**data, mode='predict')
-
-    test_step = val_step
 
 
 @MODELS.register_module()
@@ -281,15 +307,9 @@ class Embodied3DDetector(SparseFeatureFusionSingleStage3DDetector):
         img = batch_inputs_dict['imgs']
         assert img.dim() == 5 and img.shape[0] == 1, 'one scan: (1, n_views, C, H, W)'
         batch_img_metas = [ds.metainfo for ds in batch_data_samples]
-        n_prefix, V = len(points), img.shape[1]
-        assert n_prefix == len(batch_img_metas) <= V
-        img4 = img.reshape([-1] + list(img.shape)[2:]).to(self.compute_dtype)
-        if not img4.is_contiguous(memory_format=torch.channels_last):
-            img4 = img4.contiguous(memory_format=torch.channels_last)
-        img_features = self.backbone(img4)                               # per level (V, C, Hf, Wf)
-        coordinates, features = self.voxelize(points)
-        x = SP.SparseTensor(coordinates=coordinates, features=features.to(self.compute_dtype), batch_size=n_prefix)
-        x = self.backbone_3d(x)
+        assert len(points) == len(batch_img_metas) <= img.shape[1]
+        img_features = self.backbone(self.view_batch(img))               # per level (V, C, Hf, Wf)
+        x = self.sparse_levels(points)
         dev = img.device
         pad_hw = tuple(img.shape[-2:])
         metas = [pack_paint_metas([m], dev) for m in batch_img_metas]

@@ -29,9 +29,8 @@ import torch.nn.functional as F
 
 from . import sparse as SP
 from ._ffi import call, ptr, stream
-from .dense_heads import FCAF3DHeadRotMat, check_head_box_loss
-from .detectors import SparseFeatureFusionSingleStage3DDetector, detach_log_vars, parse_losses
-from .fusion import pack_paint_metas, pack_projections, paint_points
+from .dense_heads import SparseFPN, check_head_box_loss
+from .detectors import MultiModal3DModel, preprocessor_cfg
 from .geometry import (bbox_to_corners, box3d_overlap, box_corners_container, chamfer_src,
                        matrix_to_euler_angles_zxy, ortho_6d_2_mat, rotation_3d_in_euler)
 from .registry import MODELS, TASK_UTILS
@@ -628,53 +627,35 @@ class GroundingHead(nn.Module):
 
 # ======================================================================================================= sparse neck
 @MODELS.register_module()
-class MinkNeck(nn.Module):
+class MinkNeck(SparseFPN):
     """Sparse FPN with score-driven pruning (mink_neck.py:133-244); per-scan outputs are concatenated coarse -> fine."""
-
-    _make_block = staticmethod(FCAF3DHeadRotMat._make_block)
-    _make_up_block = staticmethod(FCAF3DHeadRotMat._make_up_block)
-    _run_block = FCAF3DHeadRotMat._run_block
-    _prune = FCAF3DHeadRotMat._prune
 
     def __init__(self, num_classes, in_channels, out_channels, voxel_size, pts_prune_threshold, train_cfg=None,
                  test_cfg=None, init_cfg=None):
         super().__init__()
         self.voxel_size, self.pts_prune_threshold = voxel_size, pts_prune_threshold
-        self.pruning = SP.MinkowskiPruning()
-        for i in range(len(in_channels)):
-            if i > 0:
-                setattr(self, f'up_block_{i}', self._make_up_block(in_channels[i], in_channels[i - 1]))
-            setattr(self, f'out_block_{i}', self._make_block(in_channels[i], out_channels))
+        self._init_fpn(in_channels, out_channels)
         self.conv_cls = SP.MinkowskiConvolution(out_channels, num_classes, kernel_size=1, bias=True, dimension=3)
         nn.init.normal_(self.conv_cls.kernel, std=.01)
         nn.init.constant_(self.conv_cls.bias, -4.59511985013459)
 
+    def _level(self, i: int, out: SP.SparseTensor):
+        """(per-scan features, class scores, points) of one level, and its max-class score for pruning."""
+        f = out.F
+        cls = torch.addmm(self.conv_cls.bias.to(f.dtype), f, self.conv_cls.kernel.to(f.dtype))
+        prune_score = out.replace_feature(cls.max(dim=1, keepdim=True).values.float())
+        perms = out.decomposition_permutations
+        pts = out.C[:, 1:] * self.voxel_size
+        return ([f[p] for p in perms], [cls[p] for p in perms], [pts[p] for p in perms]), prune_score
+
     def forward(self, x: List[SP.SparseTensor], batch_size: int):
-        feats, scores, points = [], [], []
-        inputs = x
-        x = inputs[-1]
-        prune_score = None
-        for i in range(len(inputs) - 1, -1, -1):
-            if i < len(inputs) - 1:
-                x = self._run_block(getattr(self, f'up_block_{i + 1}'), x)
-                x = inputs[i] + x
-                x = self._prune(x, prune_score)
-            out = self._run_block(getattr(self, f'out_block_{i}'), x)
-            f = out.F
-            cls = torch.addmm(self.conv_cls.bias.to(f.dtype), f, self.conv_cls.kernel.to(f.dtype))
-            prune_score = out.replace_feature(cls.max(dim=1, keepdim=True).values.float())
-            perms = out.decomposition_permutations
-            pts = out.C[:, 1:] * self.voxel_size
-            feats.append([f[p] for p in perms])
-            scores.append([cls[p] for p in perms])
-            points.append([pts[p] for p in perms])
-        cat = lambda lv: [torch.cat([l[b] for l in lv], 0) for b in range(batch_size)]
-        return cat(feats), cat(scores), cat(points)
+        levels = self._top_down(x, self._level)
+        return tuple([torch.cat([lv[k][b] for lv in levels], 0) for b in range(batch_size)] for k in range(3))
 
 
 # ======================================================================================================= the model
 @MODELS.register_module()
-class SparseFeatureFusion3DGrounder(nn.Module):
+class SparseFeatureFusion3DGrounder(MultiModal3DModel):
 
     def __init__(self, backbone, backbone_3d, bbox_head, neck=None, neck_3d=None, decoder=None, voxel_size=0.01,
                  num_queries=512, max_num_entities=256, coord_type='CAMERA', train_cfg=None, test_cfg=None,
@@ -682,9 +663,7 @@ class SparseFeatureFusion3DGrounder(nn.Module):
                  freeze_text_encoder=True):
         super().__init__()
         self.compute_dtype = compute_dtype
-        if isinstance(data_preprocessor, dict):
-            data_preprocessor = dict(data_preprocessor, compute_dtype=compute_dtype)
-            data_preprocessor.setdefault('type', 'Det3DDataPreprocessor')
+        data_preprocessor = preprocessor_cfg(data_preprocessor, compute_dtype)
         self.data_preprocessor = MODELS.build(data_preprocessor) if data_preprocessor is not None else None
         self.backbone = MODELS.build(backbone)
         self.backbone_3d = MODELS.build(backbone_3d)
@@ -704,27 +683,12 @@ class SparseFeatureFusion3DGrounder(nn.Module):
         self.text_feat_map = nn.Linear(self.text_encoder.config.hidden_size, self.embed_dims, bias=True)
 
     # ---- features ---------------------------------------------------------------------------------------------------
-    voxelize = SparseFeatureFusionSingleStage3DDetector.voxelize
-
     def extract_feat(self, batch_inputs_dict, batch_data_samples):
-        points = batch_inputs_dict['points']
         img = batch_inputs_dict['imgs']
-        metas_list = [ds.metainfo for ds in batch_data_samples]
-        dev = points[0].device
-        B, V = img.shape[:2]
-        img4 = img.reshape([-1] + list(img.shape)[2:]).to(self.compute_dtype)
-        if not img4.is_contiguous(memory_format=torch.channels_last):
-            img4 = img4.contiguous(memory_format=torch.channels_last)
-        img_features = self.backbone(img4)
-        coords, feats = self.voxelize(points)
-        x = SP.SparseTensor(coordinates=coords, features=feats.to(self.compute_dtype), batch_size=len(points))
-        x = self.backbone_3d(x)
-        metas = pack_paint_metas(metas_list, dev)
-        proj = pack_projections(metas_list, self.coord_type, dev)
-        for li in range(len(x)):
-            painted = paint_points(img_features[li], x[li].C, metas, proj, self.voxel_size, tuple(img.shape[-2:]), V)
-            x[li] = x[li].replace_feature(torch.cat([x[li].F, painted.to(x[li].F.dtype)], 1))
-        return self.neck_3d(x, B)
+        img_features = self.backbone(self.view_batch(img))
+        x = self.sparse_levels(batch_inputs_dict['points'])
+        self.paint_levels(x, img_features, img, [ds.metainfo for ds in batch_data_samples])
+        return self.neck_3d(x, img.shape[0])
 
     # ---- text -------------------------------------------------------------------------------------------------------
     def create_positive_map(self, tokenized, tokens_positive, batch_idx):
@@ -830,31 +794,3 @@ class SparseFeatureFusion3DGrounder(nn.Module):
         for ds, r in zip(batch_data_samples, results):
             ds.pred_instances_3d = r
         return batch_data_samples
-
-    def forward(self, inputs, data_samples=None, mode='tensor', **kwargs):
-        if self.compute_dtype == torch.float32:
-            # fp32 = the parity arithmetic: library contractions stay out of TF32 in forward AND backward
-            from .precision import fence_losses, fp32_exact
-            with fp32_exact():
-                return fence_losses(self._forward(inputs, data_samples, mode, **kwargs))
-        return self._forward(inputs, data_samples, mode, **kwargs)
-
-    def _forward(self, inputs, data_samples, mode, **kwargs):
-        if mode == 'loss':
-            return self.loss(inputs, data_samples, **kwargs)
-        if mode == 'predict':
-            return self.predict(inputs, data_samples, **kwargs)
-        raise RuntimeError(f'Invalid mode "{mode}". Only supports loss, predict and tensor mode')
-
-    def train_step(self, data, optim_wrapper):
-        data = self.data_preprocessor(data, True)
-        loss, log_vars = parse_losses(self(**data, mode='loss'))
-        optim_wrapper.update_params(loss)
-        return detach_log_vars(log_vars)
-
-    @torch.no_grad()
-    def val_step(self, data):
-        data = self.data_preprocessor(data, False)
-        return self(**data, mode='predict')
-
-    test_step = val_step

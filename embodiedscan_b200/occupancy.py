@@ -6,8 +6,9 @@ SurroundOcc losses (models/losses/occ_loss.py:7-141).
 
 Shares the front half with the detector — voxel hashing, MinkResNet34 and the point-painting kernel (here on the prior
 grid's fp32 voxel centres) all run in libesb200.so. The dense Conv3d FPN is the one tensor-core-bound stage of the named
-configs (~4 TFLOP/scan); this round it is evaluated by the library convolution (cuDNN) in channels-last-3d bf16 — the
-wgmma implicit-GEMM Conv3d is listed in DESIGN.md §7.
+configs (~4 TFLOP/scan); in bf16 it runs channels-last-3d on the library's TMA + wgmma implicit-GEMM convolutions
+(``esb_conv3d_tma_*``, DESIGN.md row a14); only the fp32 parity arithmetic and channel counts those kernels do not tile
+stay on the library Conv3d (``_tma3d_ok``).
 """
 from typing import List, Optional
 
@@ -17,7 +18,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import sparse as SP
-from .detectors import detach_log_vars, parse_losses
+from .detectors import MultiModal3DModel, preprocessor_cfg
 from .fusion import pack_paint_metas, pack_projections, paint_float_points
 from .registry import MODELS, TASK_UTILS
 
@@ -378,16 +379,14 @@ class ImVoxelOccHead(nn.Module):
 
 
 @MODELS.register_module()
-class DenseFusionOccPredictor(nn.Module):
+class DenseFusionOccPredictor(MultiModal3DModel):
 
     def __init__(self, backbone, backbone_3d, neck, neck_3d, bbox_head, prior_generator, n_voxels, coord_type,
                  use_valid_mask=True, use_xyz_feat=False, point_cloud_range=None, train_cfg=None, test_cfg=None,
                  data_preprocessor=None, init_cfg=None, compute_dtype=torch.float32):
         super().__init__()
         self.compute_dtype = compute_dtype
-        if isinstance(data_preprocessor, dict):
-            data_preprocessor = dict(data_preprocessor, compute_dtype=compute_dtype)
-            data_preprocessor.setdefault('type', 'Det3DDataPreprocessor')
+        data_preprocessor = preprocessor_cfg(data_preprocessor, compute_dtype)
         self.data_preprocessor = MODELS.build(data_preprocessor) if data_preprocessor is not None else None
         self.backbone = MODELS.build(backbone)
         self.backbone_3d = MODELS.build(backbone_3d)
@@ -411,10 +410,7 @@ class DenseFusionOccPredictor(nn.Module):
         metas_list = [ds.metainfo for ds in batch_data_samples]
         B, V = img.shape[:2]
         dev = img.device
-        img4 = img.reshape([-1] + list(img.shape)[2:]).to(self.compute_dtype)
-        if not img4.is_contiguous(memory_format=torch.channels_last):
-            img4 = img4.contiguous(memory_format=torch.channels_last)
-        feat2d = self.neck(self.backbone(img4))[0]                     # (B*V, 256, H/4, W/4)
+        feat2d = self.neck(self.backbone(self.view_batch(img)))[0]     # (B*V, 256, H/4, W/4)
 
         prior = self.prior_generator.grid_anchors([self.n_voxels[::-1]], device=dev)[0][:, :3]
         if 'origin' in metas_list[0]['depth2img']:
@@ -429,27 +425,15 @@ class DenseFusionOccPredictor(nn.Module):
         img_volume = vol.view([B] + self.n_voxels[::-1] + [-1]).permute(0, 4, 3, 2, 1)          # (B, C, X, Y, Z)
         valid_preds = ~torch.all(img_volume == 0, dim=1, keepdim=True)
 
-        # sparse branch: ((p - range_min) / voxel_size) floored, clamped into the grid (dense_fusion_occ.py:224-245)
         points = batch_inputs_dict['points']
         assert len(points) == 1, 'Only support batch size 1 for now!!'
-        vs = prior.new_tensor(self.voxel_size)
-        lo = prior.new_tensor(self.point_cloud_range[:3])
-        coords, feats = [], []
-        for b, p in enumerate(points):
-            q = torch.floor((p[:, :3].float() - lo) / vs).to(torch.int32)
-            hi = torch.tensor([n * self.voxel_stride - 1 for n in self.n_voxels], dtype=torch.int32, device=dev)
-            q = torch.minimum(torch.clamp(q, min=0), hi)
-            coords.append(torch.cat([torch.full((q.shape[0], 1), b, dtype=torch.int32, device=dev), q], 1))
-            feats.append(p.float() if self.use_xyz_feat else p[:, 3:].float())
-        x = SP.SparseTensor(coordinates=torch.cat(coords), features=torch.cat(feats).to(self.compute_dtype),
-                            batch_size=len(points))
-        last = self.backbone_3d(x)[-1]
-        point_volume, _, _ = last.dense((1, last.F.shape[-1], *self.n_voxels), min_coordinate=[0, 0, 0])
+        point_volume = self.sparse_volume(points, prior)
         fused = torch.cat([img_volume.to(self.compute_dtype), point_volume], dim=1)
         return self.neck_3d(fused.contiguous(memory_format=torch.channels_last_3d)), valid_preds.float()
 
     def sparse_volume(self, points, prior):
-        """MinkResNet over the clamped voxel grid -> dense (B, C, X, Y, Z) volume of its coarsest level."""
+        """MinkResNet over the voxel grid -> dense (B, C, X, Y, Z) volume of its coarsest level. Points are voxelised as
+        ((p - range_min) / voxel_size) floored and clamped into the grid (dense_fusion_occ.py:224-245)."""
         dev = prior.device
         vs = prior.new_tensor(self.voxel_size)
         lo = prior.new_tensor(self.point_cloud_range[:3])
@@ -476,34 +460,6 @@ class DenseFusionOccPredictor(nn.Module):
             ds.pred_occupancy = pred[i]
         return batch_data_samples
 
-    def forward(self, inputs, data_samples=None, mode='tensor', **kwargs):
-        if self.compute_dtype == torch.float32:
-            # fp32 = the parity arithmetic: library contractions stay out of TF32 in forward AND backward
-            from .precision import fence_losses, fp32_exact
-            with fp32_exact():
-                return fence_losses(self._forward(inputs, data_samples, mode, **kwargs))
-        return self._forward(inputs, data_samples, mode, **kwargs)
-
-    def _forward(self, inputs, data_samples, mode, **kwargs):
-        if mode == 'loss':
-            return self.loss(inputs, data_samples, **kwargs)
-        if mode == 'predict':
-            return self.predict(inputs, data_samples, **kwargs)
-        raise RuntimeError(f'Invalid mode "{mode}". Only supports loss and predict mode')
-
-    def train_step(self, data, optim_wrapper):
-        data = self.data_preprocessor(data, True)
-        loss, log_vars = parse_losses(self(**data, mode='loss'))
-        optim_wrapper.update_params(loss)
-        return detach_log_vars(log_vars)
-
-    @torch.no_grad()
-    def val_step(self, data):
-        data = self.data_preprocessor(data, False)
-        return self(**data, mode='predict')
-
-    test_step = val_step
-
 
 @MODELS.register_module()
 class EmbodiedOccPredictor(DenseFusionOccPredictor):
@@ -519,10 +475,7 @@ class EmbodiedOccPredictor(DenseFusionOccPredictor):
         V, dev = img.shape[1], img.device
         n_prefix = len(metas_list)
         assert n_prefix <= V
-        img4 = img.reshape([-1] + list(img.shape)[2:]).to(self.compute_dtype)
-        if not img4.is_contiguous(memory_format=torch.channels_last):
-            img4 = img4.contiguous(memory_format=torch.channels_last)
-        feat2d = self.neck(self.backbone(img4))[0]                      # (V, C, H/4, W/4)
+        feat2d = self.neck(self.backbone(self.view_batch(img)))[0]     # (V, C, H/4, W/4)
         if not feat2d.is_contiguous(memory_format=torch.channels_last):
             feat2d = feat2d.contiguous(memory_format=torch.channels_last)
         prior = self.prior_generator.grid_anchors([self.n_voxels[::-1]], device=dev)[0][:, :3]
