@@ -74,7 +74,7 @@ SIGNATURES = {
     'esb_unproject_depth_workspace_bytes': ('iii', 'z'),
     'esb_unproject_depth': ('piiifpppppzp', 'i'),
     'esb_grad_clip_coef': ('pqffpp', 'i'),
-    'esb_adamw_step': ('pppppqfffffifpp', 'i'),
+    'esb_adamw_step_groups': ('ppppppiqfffifpp', 'i'),
     'esb_cast_f32_to_bf16': ('ppqp', 'i'),
 }
 
@@ -87,7 +87,7 @@ KERNELS_PER_CALL = {
     'esb_spconv_wgrad': 1, 'esb_maxpool_fwd': 1, 'esb_maxpool_bwd': 1, 'esb_norm_fwd': 5, 'esb_norm_apply': 1,
     'esb_norm_bwd': 2, 'esb_batchnorm_fwd_fused': 2, 'esb_paint_fwd': 1, 'esb_paint_bwd': 1, 'esb_fcaf3d_targets': 5,
     'esb_focal_loss_fwd': 1, 'esb_focal_loss_bwd': 1, 'esb_nms_bev_segmented': 1, 'esb_iou_bev_pairwise': 1,
-    'esb_img_normalize': 1, 'esb_unproject_depth': 3, 'esb_grad_clip_coef': 2, 'esb_adamw_step': 1,
+    'esb_img_normalize': 1, 'esb_unproject_depth': 3, 'esb_grad_clip_coef': 2, 'esb_adamw_step_groups': 1,
     'esb_cast_f32_to_bf16': 1, 'esb_spconv_tc_fwd': 1, 'esb_spconv_tc_wgrad': 1, 'esb_kmap_tile_masks': 1,
     'esb_chamfer_fwd': 2, 'esb_chamfer_bwd': 4, 'esb_nms3d_9dof': 2,
 }

@@ -7,6 +7,7 @@ ranks, the only bulk collective is the gradient SUM (averaged inside the AdamW k
 """
 from typing import List, Optional
 
+import numpy as np
 import torch
 import torch.distributed as dist
 import torch.nn as nn
@@ -137,36 +138,176 @@ class DataParallelReducer:
         self.reset()
 
 
-class FusedAdamW:
-    """AdamW + global-norm clipping over the arena: two kernel launches per step, no host sync."""
+def custom_key(name: str, custom_keys: dict):
+    """The `paramwise_cfg.custom_keys` entry that applies to parameter `name`, or None: mmengine's
+    DefaultOptimWrapperConstructor takes the longest key contained in the name (equal lengths: alphabetical order)."""
+    for k in sorted(sorted(custom_keys), key=len, reverse=True):
+        if k in name:
+            return custom_keys[k]
+    return None
 
-    def __init__(self, arena: FlatArena, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-4, max_norm=10.0,
-                 world_size: int = 1, lr_mult: Optional[torch.Tensor] = None):
-        self.arena, self.lr, self.betas, self.eps, self.wd, self.max_norm = arena, lr, betas, eps, weight_decay, max_norm
-        self.world = world_size
-        self.lr_mult = lr_mult                       # per-element learning-rate multiplier over the arena, or None
-        dev = arena.flat.device
+
+def param_groups(model: nn.Module, lr: float, weight_decay: float, paramwise_cfg: Optional[dict] = None):
+    """torch parameter groups laid out as mmengine's DefaultOptimWrapperConstructor lays them out for the same arguments,
+    so that group and parameter indices line up with the optimizer state of an mmengine checkpoint: without
+    `paramwise_cfg` one group of `model.parameters()`; with it one group per parameter in `named_parameters()` order,
+    where a matching `custom_keys` entry sets `lr = lr * lr_mult` and `weight_decay = weight_decay * decay_mult`. Frozen
+    parameters get a group of their own without overrides. (Other `paramwise_cfg` keys are not supported.)"""
+    if not paramwise_cfg:
+        return [{'params': list(model.parameters())}]
+    keys = paramwise_cfg.get('custom_keys') or {}
+    groups = []
+    for name, p in model.named_parameters():
+        g = {'params': [p]}
+        hit = custom_key(name, keys) if p.requires_grad else None
+        if hit is not None:
+            g['lr'] = lr * hit.get('lr_mult', 1.)
+            g['weight_decay'] = weight_decay * hit.get('decay_mult', 1.)
+        groups.append(g)
+    return groups
+
+
+class FusedAdamW(torch.optim.Optimizer):
+    """torch.optim.AdamW + global-norm clipping over the arena: two kernel launches per step, no host sync.
+
+    A torch Optimizer with torch AdamW's group keys, so learning-rate schedulers (torch's and mmengine's) attach to it and
+    write `group['lr']`, which the next `step()` reads. Every trainable parameter lives in `arena`; parameters outside it
+    (frozen) sit in their groups without state. The moments `m`, `v` are arena-shaped; one step count serves all
+    parameters. `state_dict()` / `load_state_dict()` speak torch AdamW's format, with two differences: the parameters of a
+    group whose lr is 0 keep their moments (torch AdamW would still update them), and a parameter that has no state in a
+    loaded dict (torch had never seen its gradient) starts from zero moments under the shared step count."""
+
+    def __init__(self, params, arena: FlatArena, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-4,
+                 max_norm=10.0, world_size: int = 1, lr_mult: Optional[torch.Tensor] = None):
+        # torch AdamW's defaults (and its checks of the values), so the groups carry exactly its keys
+        defaults = torch.optim.AdamW([torch.zeros(1, requires_grad=True)], lr=lr, betas=betas, eps=eps,
+                                     weight_decay=weight_decay).defaults
+        super().__init__(params, defaults)
+        self.arena, self.max_norm, self.world = arena, max_norm, world_size
+        self.lr_mult = lr_mult                       # per-element learning-rate multiplier at construction, or None
         self.m = torch.zeros_like(arena.flat)
         self.v = torch.zeros_like(arena.flat)
-        self.state = torch.zeros(3, dtype=torch.float32, device=dev)   # sumsq, norm, clip coefficient
+        self.clip_state = torch.zeros(3, dtype=torch.float32, device=arena.flat.device)   # sumsq, norm, clip coefficient
         self.step_count = 0
+        self._offset = {id(p): o for p, o in zip(arena.params, arena.offsets)}
+        in_groups = {id(p) for g in self.param_groups for p in g['params']}
+        if not self._offset.keys() <= in_groups:
+            raise ValueError('FusedAdamW: every arena parameter must be in a parameter group')
+        for g in self.param_groups:
+            for p in g['params']:
+                if p.requires_grad and id(p) not in self._offset:
+                    raise ValueError('FusedAdamW: a trainable parameter of the groups has no arena slot')
+        # the kernel's group table: the groups that hold arena parameters, in order
+        self._slots = [k for k, g in enumerate(self.param_groups) if any(id(p) in self._offset for p in g['params'])]
+        self.group_of = None                         # (numel,) uint16 slot of every arena element, several slots only
+        if len(self._slots) > 1:
+            idx = np.zeros(arena.numel, dtype=np.uint16)
+            for s, k in enumerate(self._slots):
+                for p in self.param_groups[k]['params']:
+                    o = self._offset.get(id(p))
+                    if o is not None:
+                        idx[o:o + p.numel()] = s
+            self.group_of = torch.from_numpy(idx).to(arena.flat.device)
 
-    def step(self):
+    def step(self, closure=None):
+        if closure is not None:
+            raise ValueError('FusedAdamW.step takes no closure')
+        lr_wd = []
+        betas, eps = tuple(self.param_groups[self._slots[0]]['betas']), self.param_groups[self._slots[0]]['eps']
+        for k in self._slots:
+            g = self.param_groups[k]
+            if tuple(g['betas']) != betas or g['eps'] != eps:
+                raise ValueError('FusedAdamW: all parameter groups must share betas and eps')
+            lr_wd += (float(g['lr']), float(g['weight_decay']))
+        lr_wd = torch.tensor(lr_wd, dtype=torch.float32)    # host memory: the kernel launch carries the values
         a = self.arena
         self.step_count += 1
         ws = 1.0 / self.world                         # arena.grad holds the SUM over ranks
         call('esb_grad_clip_coef', ptr(a.grad), a.numel, float(self.max_norm if self.max_norm else 0.), ws,
-             ptr(self.state), stream())
-        call('esb_adamw_step', ptr(a.flat), ptr(a.grad), ptr(self.m), ptr(self.v), ptr(self.lr_mult), a.numel, self.lr, self.betas[0],
-             self.betas[1], self.eps, self.wd, self.step_count, ws, ptr(self.state), stream())
+             ptr(self.clip_state), stream())
+        call('esb_adamw_step_groups', ptr(a.flat), ptr(a.grad), ptr(self.m), ptr(self.v), ptr(self.group_of),
+             ptr(lr_wd), len(self._slots), a.numel, float(betas[0]), float(betas[1]), float(eps), self.step_count, ws,
+             ptr(self.clip_state), stream())
+
+    def zero_grad(self, set_to_none: bool = True):
+        """Zero the gradient arena. The parameters' `.grad` stay views of it whatever `set_to_none` says."""
+        self.arena.zero_grad()
+
+    def state_dict(self):
+        """torch AdamW's format. Parameters are numbered across groups in order; `exp_avg` / `exp_avg_sq` are views of the
+        arena's moments (torch's own state_dict also returns its live state tensors)."""
+        state, groups, index = {}, [], 0
+        for g in self.param_groups:
+            packed = {k: v for k, v in g.items() if k != 'params'}
+            packed['params'] = list(range(index, index + len(g['params'])))
+            index += len(g['params'])
+            for i, p in zip(packed['params'], g['params']):
+                o = self._offset.get(id(p))
+                if o is not None and self.step_count > 0:
+                    state[i] = {'step': torch.tensor(float(self.step_count), dtype=torch.float32),
+                                'exp_avg': self.m[o:o + p.numel()].view_as(p),
+                                'exp_avg_sq': self.v[o:o + p.numel()].view_as(p)}
+            groups.append(packed)
+        return {'state': state, 'param_groups': groups}
+
+    def load_state_dict(self, state_dict):
+        """Load a torch AdamW state dict (written by torch.optim.AdamW, by this class, or by mmengine's
+        OptimWrapper.state_dict(), the 'optimizer' entry of a checkpoint) for the same groups: the moments are copied
+        into the arena on the current stream, the step count and the groups' lr, initial_lr, weight_decay, betas and eps
+        are adopted, and the bf16 shadow is refreshed (a resume loads the model weights, which land in the arena, first).
+        Raises ValueError, before changing anything, if the group count, the parameters per group, a moment's shape or
+        the steps of the parameters disagree."""
+        saved = state_dict['param_groups']
+        if len(saved) != len(self.param_groups):
+            raise ValueError(f'FusedAdamW.load_state_dict: {len(saved)} parameter groups, expected '
+                             f'{len(self.param_groups)}')
+        moments, steps = [], set()
+        for k, (g, s) in enumerate(zip(self.param_groups, saved)):
+            if len(s['params']) != len(g['params']):
+                raise ValueError(f'FusedAdamW.load_state_dict: group {k} holds {len(s["params"])} parameters, '
+                                 f'expected {len(g["params"])}')
+            if s.get('amsgrad') or s.get('maximize'):
+                raise ValueError('FusedAdamW.load_state_dict: amsgrad / maximize AdamW states are not supported')
+            for p, i in zip(g['params'], s['params']):
+                o = self._offset.get(id(p))
+                if o is None:
+                    continue
+                st = state_dict['state'].get(i)
+                if st is None:
+                    moments.append((p, o, None, None))
+                    continue
+                for key in ('exp_avg', 'exp_avg_sq'):
+                    if tuple(st[key].shape) != tuple(p.shape):
+                        raise ValueError(f'FusedAdamW.load_state_dict: {key} of parameter {i} has shape '
+                                         f'{tuple(st[key].shape)}, expected {tuple(p.shape)}')
+                steps.add(float(st['step']))
+                moments.append((p, o, st['exp_avg'], st['exp_avg_sq']))
+        if len(steps) > 1:
+            raise ValueError(f'FusedAdamW.load_state_dict: the parameters disagree on the step count {sorted(steps)}')
+        for p, o, exp_avg, exp_avg_sq in moments:
+            n = p.numel()
+            if exp_avg is None:
+                self.m[o:o + n].zero_()
+                self.v[o:o + n].zero_()
+            else:
+                self.m[o:o + n].copy_(exp_avg.reshape(-1))
+                self.v[o:o + n].copy_(exp_avg_sq.reshape(-1))
+        self.step_count = int(steps.pop()) if steps else 0
+        for g, s in zip(self.param_groups, saved):
+            for key in ('lr', 'initial_lr', 'weight_decay', 'betas', 'eps'):
+                if key in s:
+                    g[key] = s[key]
+        self.arena.refresh_bf16()
 
     @property
     def grad_norm(self):
-        return self.state[1]
+        return self.clip_state[1]
 
 
 class OptimWrapper:
-    """``update_params(loss)`` of mmengine's OptimWrapper for the arena optimiser."""
+    """mmengine's OptimWrapper interface (`update_params(loss)`, `backward`, `step`, `zero_grad`, `param_groups`,
+    `get_lr`, `get_momentum`, `state_dict`, `load_state_dict`) for the arena optimiser `self.optimizer` (FusedAdamW),
+    whose groups follow mmengine's `paramwise_cfg` layout. Schedulers attach to `self.optimizer`."""
 
     def __init__(self, model: nn.Module, lr=1e-3, weight_decay=1e-4, max_norm=10.0, process_group=None,
                  bucket_bytes: int = 64 << 20, max_run_ahead: int = 1, paramwise_cfg: Optional[dict] = None,
@@ -192,32 +333,59 @@ class OptimWrapper:
         self.arena = FlatArena(model, bucket_bytes)
         world = dist.get_world_size(process_group) if dist.is_initialized() else 1
         self.reducer = DataParallelReducer(self.arena, process_group)
-        self.optimizer = FusedAdamW(self.arena, lr=lr, weight_decay=weight_decay, max_norm=max_norm, world_size=world,
+        self.optimizer = FusedAdamW(param_groups(model, lr, weight_decay, paramwise_cfg), self.arena, lr=lr,
+                                    weight_decay=weight_decay, max_norm=max_norm, world_size=world,
                                     lr_mult=self._lr_mult(model, paramwise_cfg))
         self.arena.zero_grad()
 
     def _lr_mult(self, model, paramwise_cfg):
         """mmengine `paramwise_cfg=dict(custom_keys={name_substring: dict(lr_mult=...)})` (the grounding config scales the
         decoder by 0.1 and freezes the text encoder with 0.0: configs/grounding/mv-grounding_8xb12_embodiedscan-vg-9dof.py)
-        as ONE per-element multiplier over the arena, consumed by the fused AdamW kernel. The longest matching key wins."""
+        as ONE per-element multiplier over the arena at construction. The step itself reads each group's lr."""
         keys = (paramwise_cfg or {}).get('custom_keys') or {}
         if not keys:
             return None
         names = {id(p): n for n, p in model.named_parameters()}
         mult = torch.ones(self.arena.numel, dtype=torch.float32, device=self.arena.flat.device)
         for p, o in zip(self.arena.params, self.arena.offsets):
-            name = names.get(id(p), '')
-            hit = [k for k in keys if k in name]
-            if hit:
-                mult[o:o + p.numel()] = float(keys[max(hit, key=len)].get('lr_mult', 1.0))
+            hit = custom_key(names.get(id(p), ''), keys)
+            if hit is not None:
+                mult[o:o + p.numel()] = float(hit.get('lr_mult', 1.0))
         return mult
 
-    def update_params(self, loss: torch.Tensor):
+    # what mmengine's hooks and Runner call on an optim wrapper
+    @property
+    def param_groups(self):
+        return self.optimizer.param_groups
+
+    def get_lr(self):
+        return {'lr': [g['lr'] for g in self.param_groups]}
+
+    def get_momentum(self):
+        return {'momentum': [g['betas'][0] for g in self.param_groups]}
+
+    def state_dict(self):
+        return self.optimizer.state_dict()
+
+    def load_state_dict(self, state_dict):
+        self.optimizer.load_state_dict(state_dict)
+
+    def backward(self, loss: torch.Tensor):
         loss.backward()
+
+    def step(self):
+        """All-reduce what is left, clip + AdamW, refresh the bf16 shadow."""
         self.reducer.finish()
         self.optimizer.step()
         self.arena.refresh_bf16()
+
+    def zero_grad(self):
         self.arena.zero_grad()
+
+    def update_params(self, loss: torch.Tensor):
+        self.backward(loss)
+        self.step()
+        self.zero_grad()
         self._updates += 1
         if self.gc_interval and self._updates % self.gc_interval == 0:
             import gc

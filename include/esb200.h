@@ -245,11 +245,16 @@ size_t esb_unproject_depth_workspace_bytes(int V, int H, int W);
 int esb_unproject_depth(const unsigned short* depth, int V, int H, int W, float depth_shift, const float* mats,
                         float* out, int* view_of, int* count_dev, void* ws, size_t ws_bytes, void* stream);
 
-/* ---- optimiser step over the flat parameter arena (AdamW + clip_grad; cfg :219-223) ----------------------------- */
+/* ---- optimiser step over the flat parameter arena (AdamW + clip_grad; cfg :219-223) -----------------------------
+ * esb_adamw_step_groups: one launch. lr_wd_host: n_groups (lr, weight_decay) pairs in host memory, copied into the
+ * launch (1 <= n_groups <= 2048, else ESB_EINVAL). group_of: (n,) uint16 group of every element, each < n_groups; null
+ * exactly when n_groups == 1. Elements of a group whose lr is 0 are left untouched (parameter and moments).
+ * grad_scale * clip_state[2] (esb_grad_clip_coef) scales the gradient. */
 int esb_grad_clip_coef(const float* grad, long long n, float max_norm, float world_scale, float* state, void* stream);
-int esb_adamw_step(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, const float* lr_mult,
-                   long long n, float lr, float beta1, float beta2, float eps, float weight_decay, int step,
-                   float grad_scale, const float* clip_state, void* stream);
+int esb_adamw_step_groups(float* param, const float* grad, float* exp_avg, float* exp_avg_sq,
+                          const unsigned short* group_of, const float* lr_wd_host, int n_groups, long long n,
+                          float beta1, float beta2, float eps, int step, float grad_scale, const float* clip_state,
+                          void* stream);
 int esb_cast_f32_to_bf16(const float* src, void* dst, long long n, void* stream);
 
 #ifdef __cplusplus
