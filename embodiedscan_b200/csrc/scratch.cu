@@ -6,13 +6,96 @@
 
 namespace {
 
-__global__ void sum_partial_rows_kernel(const float* __restrict__ part, int n_parts, long long width, float* __restrict__ out,
-                                        int accumulate) {
-  const long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (j >= width) return;
-  float s = accumulate ? out[j] : 0.f;
-  for (int p = 0; p < n_parts; ++p) s += part[(long long)p * width + j];
-  out[j] = s;
+constexpr int kSumThreads = 256;
+constexpr int kSumLoads = 8;                          // independent loads in flight per thread and tile
+constexpr int kSumTile = kSumThreads * kSumLoads;     // floats per shared-memory tile
+
+// s + tile[0] + tile[1] + ... + tile[n - 1], in that order (1 <= n <= kSumTile). A loss sum is one such chain per tile,
+// one dependent add per part (~450k parts for the focal loss of a C2 step): the 16-byte reads of the next 16 parts are
+// issued before the adds of the current 16, and reads past n (still inside the tile) are never added.
+__device__ __forceinline__ float add_chain_contiguous(const float* __restrict__ tile, int n, float s) {
+  const float4* q = reinterpret_cast<const float4*>(tile);
+  float4 a[4];
+#pragma unroll
+  for (int u = 0; u < 4; ++u) a[u] = q[u];
+  int r = 0;
+  for (; r + 16 <= n; r += 16) {
+    const int nx = min(r + 16, kSumTile - 16) / 4;
+    float4 b[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) b[u] = q[nx + u];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      s = __fadd_rn(s, a[u].x);
+      s = __fadd_rn(s, a[u].y);
+      s = __fadd_rn(s, a[u].z);
+      s = __fadd_rn(s, a[u].w);
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) a[u] = b[u];
+  }
+  const float rest[16] = {a[0].x, a[0].y, a[0].z, a[0].w, a[1].x, a[1].y, a[1].z, a[1].w,
+                          a[2].x, a[2].y, a[2].z, a[2].w, a[3].x, a[3].y, a[3].z, a[3].w};
+#pragma unroll
+  for (int u = 0; u < 16; ++u)
+    if (r + u < n) s = __fadd_rn(s, rest[u]);
+  return s;
+}
+
+// Block b finishes the `cw` columns j = b * cw + c, c < cw (cw a power of two dividing kSumThreads). The finishers'
+// callers have few columns and many parts (a loss sum has one column and thousands of parts), so the whole block loads:
+// tiles of kSumTile / cw parts x cw columns, every thread kSumLoads independent coalesced loads, through shared memory to
+// thread c, which adds its column in part order, each add rounded on its own. The next tile is in flight in the loaders'
+// registers while the current one is added.
+__global__ void __launch_bounds__(kSumThreads) sum_partial_rows_kernel(const float* __restrict__ part, int n_parts,
+                                                                       long long width, float* __restrict__ out,
+                                                                       int accumulate, int cw) {
+  __shared__ __align__(16) float tile[kSumTile];
+  const int t = threadIdx.x;
+  const int rows = kSumTile / cw, rstep = kSumThreads / cw;
+  const int r0 = t / cw;
+  const long long j = blockIdx.x * (long long)cw + (t & (cw - 1));
+  const bool col_ok = j < width;
+  const bool adder = t < cw && col_ok;
+  float v[kSumLoads];
+  auto load = [&](int p0) {
+#pragma unroll
+    for (int k = 0; k < kSumLoads; ++k) {
+      const int p = p0 + r0 + k * rstep;
+      v[k] = col_ok && p < n_parts ? part[(long long)p * width + j] : 0.f;
+    }
+  };
+  float s = adder && accumulate ? out[j] : 0.f;
+  if (n_parts > 0) load(0);
+  for (int p0 = 0; p0 < n_parts; p0 += rows) {
+    __syncthreads();                                  // the adders are done with the previous tile
+#pragma unroll
+    for (int k = 0; k < kSumLoads; ++k) tile[t + k * kSumThreads] = v[k];   // = row r0 + k * rstep, column t % cw
+    __syncthreads();
+    if (p0 + rows < n_parts) load(p0 + rows);
+    if (adder && cw == 1) {
+      s = add_chain_contiguous(tile, min(rows, n_parts - p0), s);
+    } else if (adder) {
+      // 16 parts per group; the next group's reads (clamped inside the tile) are requested before this group's adds
+      const int n = min(rows, n_parts - p0);
+      const float* col = tile + t;
+      float a[16];
+#pragma unroll
+      for (int u = 0; u < 16; ++u) a[u] = col[min(u, n - 1) * cw];
+      int r = 0;
+      for (; r + 16 <= n; r += 16) {
+        float b[16];
+#pragma unroll
+        for (int u = 0; u < 16; ++u) b[u] = col[min(r + 16 + u, n - 1) * cw];
+#pragma unroll
+        for (int u = 0; u < 16; ++u) s = __fadd_rn(s, a[u]);
+#pragma unroll
+        for (int u = 0; u < 16; ++u) a[u] = b[u];
+      }
+      for (int u = 0; r + u < n; ++u) s = __fadd_rn(s, col[(r + u) * cw]);
+    }
+  }
+  if (adder) out[j] = s;
 }
 
 }  // namespace
@@ -72,7 +155,12 @@ cudaError_t esb_scratch_free(void* p, cudaStream_t s) { return cudaFreeAsync(p, 
 
 int esb_sum_partial_rows(const float* part, int n_parts, long long width, float* out, int accumulate, cudaStream_t s) {
   if (width == 0) return ESB_OK;
-  sum_partial_rows_kernel<<<esb_div_up(width, 256), 256, 0, s>>>(part, n_parts, width, out, accumulate);
+  // Narrow sums: 8 columns per block, so a tile is 256 parts deep and its add chain (~4 cycles per part) outlasts the
+  // next tile's load latency. Wide sums: widen the blocks until the grid is at most ~8 blocks per SM.
+  int cw = 1;
+  while (cw < 8 && cw < width) cw *= 2;
+  while (cw < kSumThreads && (width + cw - 1) / cw > 8LL * esb_sm_count()) cw *= 2;
+  sum_partial_rows_kernel<<<esb_div_up(width, cw), kSumThreads, 0, s>>>(part, n_parts, width, out, accumulate, cw);
   ESB_CUDA_LAUNCH_CHECK("sum_partial_rows_kernel");
   return ESB_OK;
 }

@@ -346,10 +346,13 @@ spconv_tc_wgrad_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16*
   }
 }
 
-// dw[k] += the partials of the chunks of offset k, in chunk order (chunks enumerate offset by offset, as in the kernel above)
+// dw[k] += the partials of the chunks of offset k, in chunk order (chunks enumerate offset by offset, as in the kernel above).
+// Thread = 4 consecutive columns of one offset (cin * cout is a multiple of 4096; the scratch partials are 16-byte aligned):
+// the 16-byte loads of 8 chunks are in flight before their in-order adds, one add chain per column.
 __global__ void spconv_wgrad_reduce_kernel(const float* __restrict__ part, const int* __restrict__ k_offsets, float* __restrict__ dw,
                                            int cin, int cout, int K, int chunk_pairs) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  constexpr int D = 8;
+  const long long e = (blockIdx.x * (long long)blockDim.x + threadIdx.x) * 4;
   const long long per_k = (long long)cin * cout;
   if (e >= per_k * K) return;
   const int k = (int)(e / per_k);
@@ -357,9 +360,25 @@ __global__ void spconv_wgrad_reduce_kernel(const float* __restrict__ part, const
   int c0 = 0;
   for (int kk = 0; kk < k; ++kk) c0 += (k_offsets[kk + 1] - k_offsets[kk] + chunk_pairs - 1) / chunk_pairs;
   const int nch = (k_offsets[k + 1] - k_offsets[k] + chunk_pairs - 1) / chunk_pairs;
-  float s = dw[e];
-  for (int c = c0; c < c0 + nch; ++c) s += part[(long long)c * per_k + j];
-  dw[e] = s;
+  float s[4] = {dw[e], dw[e + 1], dw[e + 2], dw[e + 3]};
+  const float4* src = reinterpret_cast<const float4*>(part + (long long)c0 * per_k + j);
+  const long long stride = per_k / 4;
+  for (int c = 0; c < nch; c += D) {
+    float4 v[D];
+#pragma unroll
+    for (int u = 0; u < D; ++u)
+      if (c + u < nch) v[u] = src[(c + u) * stride];
+#pragma unroll
+    for (int u = 0; u < D; ++u)
+      if (c + u < nch) {
+        s[0] = __fadd_rn(s[0], v[u].x);
+        s[1] = __fadd_rn(s[1], v[u].y);
+        s[2] = __fadd_rn(s[2], v[u].z);
+        s[3] = __fadd_rn(s[3], v[u].w);
+      }
+  }
+#pragma unroll
+  for (int q = 0; q < 4; ++q) dw[e + q] = s[q];
 }
 
 template <int N_TILE, int STAGES, bool B_MN>
@@ -467,8 +486,8 @@ extern "C" int esb_spconv_tc_wgrad(const void* x, const void* dy, const int* pai
                ? launch_wgrad<128, 3>(x, dy, pair_in, pair_out, k_offsets, part, cin, cout, K, n_chunks, chunk_pairs, stream)
                : launch_wgrad<64, 4>(x, dy, pair_in, pair_out, k_offsets, part, cin, cout, K, n_chunks, chunk_pairs, stream);
   if (rc == ESB_OK) {
-    spconv_wgrad_reduce_kernel<<<esb_div_up((long long)K * cin * cout, 256), 256, 0, stream>>>(part, k_offsets, dw, cin, cout, K,
-                                                                                             chunk_pairs);
+    spconv_wgrad_reduce_kernel<<<esb_div_up((long long)K * cin * cout / 4, 256), 256, 0, stream>>>(part, k_offsets, dw, cin, cout,
+                                                                                                 K, chunk_pairs);
   }
   ESB_CUDA_CALL(esb_scratch_free(part, stream));
   if (rc != ESB_OK) return rc;
