@@ -6,7 +6,8 @@ Host side mirrors the reference's registry / module interface; every hot operato
 from .registry import MODELS, TASK_UTILS  # noqa: F401
 from . import sparse  # noqa: F401
 from .backbones import MinkResNet, ResNet  # noqa: F401
-from .dense_heads import BBoxCDLoss, ChamferDistance, FCAF3DHeadRotMat, chamfer_distance  # noqa: F401
+from .dense_heads import (BBoxCDLoss, ChamferDistance, FCAF3DHead, FCAF3DHeadRotMat, RotatedIoU3DLoss,  # noqa: F401
+                          chamfer_distance, rotated_iou_3d)
 from .detectors import Det3DDataPreprocessor, SparseFeatureFusionSingleStage3DDetector  # noqa: F401
 from .grounding import GroundingHead, MinkNeck, SparseFeatureFusion3DGrounder  # noqa: F401
 from .occupancy import DenseFusionOccPredictor, ImVoxelOccHead, IndoorImVoxelNeck  # noqa: F401

@@ -67,6 +67,8 @@ SIGNATURES = {
     'esb_nms_bev_segmented': ('ppiifipp', 'i'),
     'esb_iou_bev_pairwise': ('pipiipp', 'i'),
     'esb_box3d_overlap': ('pipippp', 'i'),
+    'esb_rotated_iou3d_fwd': ('pipiqpp', 'i'),
+    'esb_rotated_iou3d_bwd': ('pipiqpppp', 'i'),
     'esb_nms3d_9dof_workspace_bytes': ('iii', 'z'),
     'esb_nms3d_9dof': ('pppp' + 'ii' + 'ff' + 'ii' + 'ppp' + 'zp', 'i'),
     'esb_hungarian_batch': ('ppiiippp', 'i'),

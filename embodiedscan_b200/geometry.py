@@ -51,6 +51,19 @@ def rotation_3d_in_euler(points: torch.Tensor, angles: torch.Tensor) -> torch.Te
     return torch.bmm(points, rot_t)
 
 
+def rotation_3d_in_axis(points: torch.Tensor, angles: torch.Tensor, axis: int = 2) -> torch.Tensor:
+    """points (N, M, 3) rotated counter-clockwise about z by angles (N,): x' = x cos - y sin, y' = x sin + y cos
+    (embodiedscan/structures/bbox_3d/utils.py:90-171 with clockwise=False; the same einsum). Only axis 2 is needed."""
+    if axis not in (2, -1):
+        raise NotImplementedError(f'rotation_3d_in_axis implements axis 2 only, got axis={axis}')
+    if points.shape[0] == 0:
+        return points
+    c, s = torch.cos(angles), torch.sin(angles)
+    o, z = torch.ones_like(c), torch.zeros_like(c)
+    rot_mat_t = torch.stack([torch.stack([c, s, z]), torch.stack([-s, c, z]), torch.stack([z, z, o])])
+    return torch.einsum('aij,jka->aik', points, rot_mat_t)
+
+
 _CORNER_SIGNS = None
 
 

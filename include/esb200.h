@@ -214,6 +214,15 @@ int esb_iou_bev_pairwise(const float* a, int na, const float* b, int nb, int rot
 int esb_box3d_overlap(const float* corners1, int n1, const float* corners2, int n2, float* vol, float* iou,
                       void* stream);
 
+/* ---- differentiable rotated 3D IoU of one-to-one box pairs (mmcv.ops.diff_iou_rotated_3d, the IoU behind
+ * RotatedIoU3DLoss, rotated_iou_loss.py:14-91). a (n, lda), b (n, ldb) fp32 rows (x, y, z, w, l, h, alpha, ...), z the
+ * box centre, lda, ldb >= 7; columns past 7 are ignored. fwd writes iou (n). bwd recomputes the geometry and writes
+ * grad_a / grad_b (n, 7) = grad_iou * d iou / d (x, y, z, w, l, h, alpha); grad_b may be NULL. One thread per pair, no
+ * atomics: bit-reproducible. ---- */
+int esb_rotated_iou3d_fwd(const float* a, int lda, const float* b, int ldb, long long n, float* iou, void* stream);
+int esb_rotated_iou3d_bwd(const float* a, int lda, const float* b, int ldb, long long n, const float* grad_iou,
+                          float* grad_a, float* grad_b, void* stream);
+
 /* ---- greedy NMS on the exact 9-DoF 3D IoU (the demo's final box filter `nms_filter`, demo/demo.py:84-130), batched over
  * S segments. boxes9 (M,9) = centre, size, ZXY Euler angles; scores (M); labels (M) in [0, num_classes); seg_off (S+1).
  * Candidates are already score-descending inside each segment. Walking a segment in order, a candidate is skipped when
