@@ -67,6 +67,7 @@ SIGNATURES = {
     'esb_nms_bev_segmented': ('ppiifipp', 'i'),
     'esb_iou_bev_pairwise': ('pipiipp', 'i'),
     'esb_box3d_overlap': ('pipippp', 'i'),
+    'esb_box3d_best_overlap': ('pippppppp', 'i'),
     'esb_rotated_iou3d_fwd': ('pipiqpp', 'i'),
     'esb_rotated_iou3d_bwd': ('pipiqpppp', 'i'),
     'esb_nms3d_9dof_workspace_bytes': ('iii', 'z'),

@@ -157,6 +157,25 @@ def box3d_overlap(corners1: torch.Tensor, corners2: torch.Tensor, eps: float = 1
     return vol, iou
 
 
+def box3d_best_overlap(qcorners: torch.Tensor, tcorners: torch.Tensor, tidx: torch.Tensor, qbeg: torch.Tensor,
+                       qend: torch.Tensor):
+    """Per query box i, the best 9-DoF IoU against the targets ``tidx[qbeg[i]:qend[i]]`` and the target index that gives
+    it: corners (M,8,3) and (G,8,3) as for :func:`box3d_overlap`, ``tidx`` / ``qbeg`` / ``qend`` integer CUDA tensors ->
+    (best (M,) fp32, arg (M,) int32). An empty range gives (-inf, -1). Each IoU has the bits ``box3d_overlap`` gives the
+    pair; the choice is ``torch.max``'s (a NaN wins, ties to the smallest target index). One launch (csrc/iou3d.cu)."""
+    from ._ffi import call, ptr, stream
+    assert qcorners.is_cuda, 'box3d_best_overlap runs in libesb200.so (no CPU fallback)'
+    cq, ct = qcorners.float().contiguous(), tcorners.float().contiguous()
+    tidx, qbeg, qend = (x.to(device=cq.device, dtype=torch.int32).contiguous() for x in (tidx, qbeg, qend))
+    m = cq.shape[0]
+    assert qbeg.shape == qend.shape == (m, ) and ct.shape[1:] == (8, 3) and cq.shape[1:] == (8, 3)
+    assert ct.shape[0] < 2 ** 31 and tidx.numel() < 2 ** 31
+    best = torch.empty(m, dtype=torch.float32, device=cq.device)
+    arg = torch.empty(m, dtype=torch.int32, device=cq.device)
+    call('esb_box3d_best_overlap', ptr(cq), m, ptr(ct), ptr(tidx), ptr(qbeg), ptr(qend), ptr(best), ptr(arg), stream())
+    return best, arg
+
+
 def nms3d_9dof(boxes9: torch.Tensor, scores: torch.Tensor, labels: torch.Tensor, iou_thr: float,
                score_thr: float = float('-inf'), topk_per_class=None, seg_off=None, num_classes=None):
     """Class-agnostic greedy NMS on the exact 9-DoF 3D IoU with a score threshold and a per-label cap, the semantics of

@@ -213,6 +213,12 @@ int esb_iou_bev_pairwise(const float* a, int na, const float* b, int nb, int rot
 /* ---- exact 9-DoF box IoU (pytorch3d.ops.box3d_overlap via EulerInstance3DBoxes.overlaps, euler_box3d.py:103-135) ---- */
 int esb_box3d_overlap(const float* corners1, int n1, const float* corners2, int n2, float* vol, float* iou,
                       void* stream);
+/* Best same-range overlap: query i is compared with the targets tidx[qbeg[i] .. qend[i]) only (qcorners (m,8,3),
+ * tcorners (g,8,3) fp32, tidx int32 into the g targets). best[i] = max IoU over the range (-inf when it is empty), arg[i] =
+ * the target index that gives it (-1 when empty); a NaN IoU wins, ties go to the smallest target index (torch.max's
+ * choice). Every pair is the arithmetic of esb_box3d_overlap, bit for bit; one thread per query, no atomics. */
+int esb_box3d_best_overlap(const float* qcorners, int m, const float* tcorners, const int* tidx, const int* qbeg,
+                           const int* qend, float* best, int* arg, void* stream);
 
 /* ---- differentiable rotated 3D IoU of one-to-one box pairs (mmcv.ops.diff_iou_rotated_3d, the IoU behind
  * RotatedIoU3DLoss, rotated_iou_loss.py:14-91). a (n, lda), b (n, ldb) fp32 rows (x, y, z, w, l, h, alpha, ...), z the
