@@ -118,7 +118,9 @@ class _BiasResAct(torch.autograd.Function):
                       _ffi.dtype_code(y.dtype), _ffi.stream())
         else:
             g = dy
-        return g, None, (g if ctx.has_res else None), None
+        # the bias is the folded BN shift beta - mean * scale: it needs a gradient whenever the BN affine is trainable
+        db = g.sum((0, 2, 3), dtype=torch.float32) if ctx.needs_input_grad[1] else None
+        return g, db, (g if ctx.has_res else None), None
 
 
 def ohwi(w: torch.Tensor) -> torch.Tensor:

@@ -1,5 +1,5 @@
-"""Per-element error bounds for the bf16 kernels of the sparse branch, their float64 references, and the faults the bounds
-must catch.
+"""Per-element error bounds for the bf16 kernels of the training steps, their float64 references, and the faults the
+bounds must catch.
 
 A kernel output `out` (bf16 operands, fp32 accumulation) is checked element by element against a float64 reference `ref`
 computed from the same bf16-rounded operands:
@@ -34,6 +34,15 @@ names from the SM count.
 Painting has its own constant, C_PAINT = 1.0 (the textbook one): its backward adds a handful of pairs per pixel, each
 term rounded twice (1 / count and the product) before the sum, and onto a non-zero gradient the worst ratio measured on
 the same H100 was 0.54, above C_ACC; its forward stays below C_ACC.
+
+The head, loss and elementwise kernels (tests/test_head_elementwise_bf16_gpu.py) use C_ACC too. On the same H100 SXM
+(700 W power limit) their worst ratios were: 0.0667 for the focal loss (sum and per-element gradient, fp32 and bf16
+logits, the C2-size sum included; the conditioning K(x) = 1 + e^|x| of `focal_ref` is in the element term, not in c),
+0.284 for bias_act_kernel (the fp32 cases, one rounding of x + bias; every bf16 case rounds to the reference exactly),
+0.367 for act_bwd_kernel (fp32 ELU; without its `fixed` term, reading ELU's derivative from the bf16 output would need
+c = 4.2e6), 0.152 for interp_features_kernel, and 0.0015 for the BatchNorm / InstanceNorm instances with ELU (their
+backward carrying the same `fixed` term through the normalisation's backward, `seg_norm_bwd_fixed`). The faults are
+`focal_faults_fwd`, `focal_faults_bwd`, `bias_act_faults`, `act_bwd_faults` and `interp_faults`.
 
 Nothing here imports the library: it runs on CPU tensors as well as CUDA tensors.
 """
@@ -637,3 +646,214 @@ def paint_faults(out, dfeat, ref, feat, dout):
     bwd = [(f'pairs of views {j} dropped', bad0.to(dfeat.dtype)),
            ('divisor counts every view inside the map', bad1.to(dfeat.dtype))]
     return fwd, bwd
+
+
+# ================================================================================================ head, loss, elementwise
+# The remaining floating-point kernels of the bf16 steps (tests/test_head_elementwise_bf16_gpu.py): the sigmoid focal loss,
+# the 2-D backbone's bias + residual + activation epilogue and its backward, and the interpolation of `_prune`. The others
+# of that module (gather2_rows, img_normalize, cast) are held bit for bit.
+FLT_MIN = 1.17549435e-38
+LOG_FLT_MIN = math.log(FLT_MIN)
+FOCAL_ELEM = 64
+
+
+def focal_ref(x, target, row_w, gamma, alpha, scale=1.0):
+    """mmcv's sigmoid focal loss (csrc/head.cu) in float64 on the same logits x (n, C): per element
+      positive (target[r] == c): l = -alpha (1-p)^gamma log(max(p, FLT_MIN)),
+                                 g = -alpha (1-p)^gamma (1 - p - gamma p log(max(p, FLT_MIN)))
+      negative:                  l = -(1-alpha) p^gamma log(max(1-p, FLT_MIN)),
+                                 g = -(1-alpha) p^gamma (gamma (1-p) log(max(1-p, FLT_MIN)) - p)
+    each times row_w[r] (and g times `scale`). A target outside [0, C) (-1 or >= C) has no positive column.
+
+    Conditioning: the kernel evaluates p = 1 / (1 + expf(-x)) to a few fp32 roundings of p, and 1 - p in fp32 inherits that
+    absolute error, i.e. a relative error of (p / (1 - p)) 2^-24 = e^x 2^-24 per rounding; (1-p)^gamma, and log p near
+    p = 1 (magnitude ~ e^-x), carry it into the element. At the other end, x << 0, 1 - p is accurate but near 1, and
+    logf(1 - p) (magnitude ~ p ~ e^x) is off by the absolute rounding of 1 - p, a relative 2^-24 e^-x. So an element is off
+    by a relative 2^-24 FOCAL_ELEM K(x) with K(x) = 1 + e^|x|; FOCAL_ELEM = 64 covers the ~10 roundings of an element
+    (expf's 2 ulp included) with each term's conditioning. Returns dict(l, g, K) in float64."""
+    xd = x.double()
+    p, q = torch.sigmoid(xd), torch.sigmoid(-xd)             # q = 1 - p without cancellation
+    C = x.shape[1]
+    pos = target.view(-1, 1).to(x.device) == torch.arange(C, device=x.device).view(1, -1)
+    lp, lq = torch.log(p.clamp(min=FLT_MIN)), torch.log(q.clamp(min=FLT_MIN))
+    l = torch.where(pos, -alpha * q ** gamma * lp, -(1 - alpha) * p ** gamma * lq)
+    g = torch.where(pos, -alpha * q ** gamma * (q - gamma * p * lp), -(1 - alpha) * p ** gamma * (gamma * q * lq - p))
+    w = row_w.double().view(-1, 1)
+    return dict(l=l * w, g=g * w * scale, K=1 + torch.exp(xd.abs()))
+
+
+def focal_operands(n, C, gen, wide=False):
+    """Logits (n, C) fp32, targets (n,) int64 and row weights (n,) fp32 for the focal cases. Targets: a third -1, a third
+    >= C (no positive either way), a third in range. Row weights of unequal size from 0.05 to 1, the last row 40 (so the
+    last, partial, block of the sum carries weight). 'typical' logits are those of a training head: negatives N(-2, 2)
+    within [-12, 6], positives N(3, 2) within [-4, 12]; wide=True draws every logit uniformly from [-12, 12], which puts
+    negatives where the fp32 1 - p is worst conditioned (K up to e^12)."""
+    kind = torch.randint(0, 3, (n, ), generator=gen)
+    target = torch.where(kind == 0, -1, torch.where(kind == 1, C + torch.randint(0, 5, (n, ), generator=gen),
+                                                    torch.randint(0, C, (n, ), generator=gen)))
+    if wide:
+        x = torch.rand(n, C, generator=gen) * 24 - 12
+    else:
+        x = (torch.randn(n, C, generator=gen) * 2 - 2).clamp(-12, 6)
+        pos = torch.nonzero(kind == 2).squeeze(1)
+        x[pos, target[pos]] = (torch.randn(pos.numel(), generator=gen) * 2 + 3).clamp(-4, 12)
+    w = torch.rand(n, generator=gen) * 0.95 + 0.05
+    w[-1] = 40.0
+    return x, target.long(), w
+
+
+def focal_sum_bound(ref, n_blocks):
+    """(sum, A) of the focal loss sum for the bound with n_red = 1: each element rounded as focal_ref says, then added
+    through the 256-wide block (5 shuffle levels, 8 warp partials) and the ordered sum of the n_blocks partials."""
+    la = ref['l'].abs()
+    return ref['l'].sum(), (5 + 8 + n_blocks) * la.sum() + FOCAL_ELEM * (ref['K'] * la).sum()
+
+
+def focal_faults_fwd(x, target, row_w, gamma, alpha, total):
+    """Copies of a correct loss sum `total` with one fault each: alpha swapped between the classes, the row with the
+    largest contribution dropped, the last partial 256-element block dropped, gamma taken as 1, and (C > 1) the positive
+    column off by one."""
+    n, C = x.shape
+    ref = focal_ref(x, target, row_w, gamma, alpha)['l']
+    t1 = torch.where((target >= 0) & (target < C - 1), target + 1, target)
+    row = ref.sum(1)
+    last = n * C // 256 * 256
+    assert last < n * C, 'the last block must be partial'
+    d = total.double()
+    faults = [('alpha swapped', d - ref.sum() + focal_ref(x, target, row_w, gamma, 1 - alpha)['l'].sum()),
+              ('largest row dropped', d - row[row.abs().argmax()]),
+              ('last partial block dropped', d - ref.reshape(-1)[last:].sum()),
+              ('gamma taken as 1', d - ref.sum() + focal_ref(x, target, row_w, 1.0, alpha)['l'].sum())]
+    if C > 1:
+        faults.append(('positive column off by one', d - ref.sum() + focal_ref(x, t1, row_w, gamma, alpha)['l'].sum()))
+    return faults
+
+
+def focal_faults_bwd(x, target, row_w, gamma, alpha, scale, grad):
+    """A correct focal gradient with: alpha swapped, the row weights dropped, gamma taken as 1, the sign flipped, `scale`
+    ignored and (C > 1) the positive column off by one."""
+    C = x.shape[1]
+    t1 = torch.where((target >= 0) & (target < C - 1), target + 1, target)
+    f = lambda **kw: focal_ref(x, kw.get('t', target), kw.get('w', row_w), kw.get('gm', gamma), kw.get('a', alpha),  # noqa: E731
+                               kw.get('s', scale))['g'].to(grad.dtype)
+    faults = [('alpha swapped', f(a=1 - alpha)), ('row weights dropped', f(w=torch.ones_like(row_w))),
+              ('gamma taken as 1', f(gm=1.0)), ('sign flipped', -grad), ('scale ignored', f(s=1.0))]
+    return faults + ([('positive column off by one', f(t=t1))] if C > 1 else [])
+
+
+def _act(z, act):
+    return z if act == 0 else (z.clamp(min=0) if act == 1 else torch.where(z > 0, z, torch.expm1(z)))
+
+
+def bias_act_ref(x, bias, res, act):
+    """y = act(x + bias[c] (+ res)) in float64 on (rows, C): (y, A, n_red). The kernel rounds the two additions (and
+    expm1f for ELU), and the output rounding applies to a value already off by those: n_red = 3 (ELU 4). Every activation
+    is 1-Lipschitz, so the error of z carries over to y. (One fp32 rounding of x + b alone needs c n_red <= 1: the fp32
+    cases measured 0.42 at n_red = 2.)"""
+    z = x.double() + bias.double().view(1, -1)
+    A = x.double().abs() + bias.double().abs().view(1, -1)
+    if res is not None:
+        z, A = z + res.double(), A + res.double().abs()
+    return _act(z, act), A, 4 if act == 2 else 3
+
+
+def bias_act_faults(y, x, bias, res, act, rows_per_block):
+    """The epilogue with the bias read one channel off, the residual dropped (when there is one), ELU / ReLU left out, and
+    the last partial block of rows not written (in place: still holding x)."""
+    dt = y.dtype
+    faults = [('bias one channel off', bias_act_ref(x, bias.roll(1), res, act)[0].to(dt))]
+    if res is not None:
+        faults.append(('residual dropped', bias_act_ref(x, bias, None, act)[0].to(dt)))
+    if act:
+        faults.append(('activation left out', bias_act_ref(x, bias, res, 0)[0].to(dt)))
+    tail = y.clone()
+    r0 = x.shape[0] // rows_per_block * rows_per_block
+    if r0 == x.shape[0]:
+        r0 -= rows_per_block
+    tail[r0:] = x[r0:]
+    faults.append(('last block of rows not written', tail))
+    return faults
+
+
+def act_bwd_ref(dy, z, y, act):
+    """dx = dy act'(z) in float64, the derivative from the float64 pre-activation z, for the kernel that reads it from the
+    stored output y (ReLU: y > 0; ELU: y > 0 ? 1 : y + 1). Returns (dx, A, n_red, fixed): the product rounds once (ELU: y + 1
+    too); `fixed` = |dy| |y - act(z)| (1 + 2^-7) is what reading the derivative from the rounded output y costs (ELU's
+    derivative is y + 1 on the negative side, so it is off by exactly the error of y; on the positive side it is 1 either
+    way; ReLU's is exact while y and z have the same sign), the factor keeping the output rounding of a value already off by
+    that much covered."""
+    zd, dyd = z.double(), dy.double()
+    d = torch.ones_like(zd) if act == 0 else ((zd > 0).double() if act == 1 else torch.where(zd > 0, 1.0, torch.exp(zd)))
+    dx = dyd * d
+    fixed = dyd.abs() * (y.double() - _act(zd, act)).abs() * (zd <= 0) * (1 + 2.0 ** -7) if act == 2 else \
+        torch.zeros_like(dx)
+    return dx, dx.abs() + fixed, 2 if act == 2 else 1, fixed
+
+
+def act_bwd_faults(dx, dy, z, act):
+    """The activation gradient with the tail (the last n % 8 elements, or the last 8) not written, ELU's derivative taken
+    as ReLU's, and the sign flipped."""
+    n = dx.numel()
+    tail = dx.clone()
+    tail[n - (n % 8 or 8):] = 0
+    faults = [('tail not written', tail), ('sign flipped', -dx)]
+    if act == 2:
+        faults.append(('ReLU derivative for ELU', (dy.double() * (z.double() > 0)).to(dx.dtype)))
+    return faults
+
+
+def seg_norm_bwd_fixed(x, F, st):
+    """How far seg_norm_bwd_ref's dx, dgamma and dbeta move when gy moves by at most F per element (gamma excluded from
+    dx: multiply by |gamma|): rstd (F + mean_s F + |xhat| mean_s(F |xhat|)), sum F |xhat|, sum F."""
+    seg, n, rs = st['seg'], st['n'], st['rs']
+    S, C = n.shape[0], x.shape[1]
+    xh = ((x.double() - st['mean'][seg]) * rs[seg]).abs()
+    P = torch.zeros((S, C), dtype=torch.float64, device=x.device)
+    mf, mfx = P.clone().index_add_(0, seg, F) / n, P.clone().index_add_(0, seg, F * xh) / n
+    return rs[seg] * (F + mf[seg] + xh * mfx[seg]), (F * xh).sum(0), F.sum(0)
+
+
+def interp_ref(coords, feats, ts, query, trunc=False):
+    """Multilinear interpolation (csrc/hash.cu::interp_features_kernel) in float64 on the same features: coords (n, 4)
+    int64 [b, x, y, z] (multiples of ts), feats (n, C), query (m, 4) int64. base = floor(q / ts) ts, frac = q / ts - floor,
+    out = sum over the 8 corners present of F[corner] w_k, w_k = product of frac or 1 - frac. Returns (out, A, n_red = 11:
+    eight products and additions plus the three roundings of a weight, the (m, 8) corner rows (-1 when absent), the (m, 8)
+    weights). trunc=True rounds q / ts towards zero instead (a fault)."""
+    import numpy as np
+    q = np.asarray(query, dtype=np.int64)
+    c = np.asarray(coords, dtype=np.int64)
+    v = q[:, 1:] / float(ts)
+    fl = np.trunc(v) if trunc else np.floor(v)
+    base = fl.astype(np.int64) * ts
+    frac = v - fl
+    off = 1 << 20
+
+    def key(a):
+        return ((a[:, 0] * (1 << 21) + a[:, 1] + off) * (1 << 21) + a[:, 2] + off) * (1 << 21) + a[:, 3] + off
+    order = np.argsort(key(c))
+    ks = key(c)[order]
+    rows = np.full((q.shape[0], 8), -1, dtype=np.int64)
+    w = np.zeros((q.shape[0], 8))
+    for k in range(8):
+        d = np.array([k & 1, (k >> 1) & 1, (k >> 2) & 1])
+        kk = key(np.concatenate([q[:, :1], base + d * ts], 1))
+        pos = np.clip(np.searchsorted(ks, kk), 0, len(ks) - 1)
+        rows[:, k] = np.where(ks[pos] == kk, order[pos], -1)
+        w[:, k] = np.prod(np.where(d.astype(bool), frac, 1 - frac), 1)
+    f = feats.double()
+    r = torch.from_numpy(rows).to(f.device)
+    wt = torch.from_numpy(w).to(f.device)
+    g = f[r.clamp(min=0)] * (r >= 0)[..., None] * wt[..., None]
+    return g.sum(1), g.abs().sum(1), 11, r, wt
+
+
+def interp_faults(out, coords, feats, ts, query):
+    """The interpolation with the last corner (k = 7) dropped, q / ts truncated towards zero instead of floored, and absent
+    corners read as row 0."""
+    ref, _, _, rows, wt = interp_ref(coords, feats, ts, query)
+    f = feats.double()
+    k7 = ref - f[rows[:, 7].clamp(min=0)] * ((rows[:, 7] >= 0) * wt[:, 7])[:, None]
+    absent = ref + ((rows < 0) * wt).sum(1, keepdim=True) * f[0][None]
+    return [('corner 7 dropped', k7.to(out.dtype)),
+            ('truncation instead of floor', interp_ref(coords, feats, ts, query, trunc=True)[0].to(out.dtype)),
+            ('absent corners read as row 0', absent.to(out.dtype))]

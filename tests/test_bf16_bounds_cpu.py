@@ -194,3 +194,79 @@ def test_bound_accepts_emulated_painting_and_rejects_its_faults():
     assert len(fwd_f) == 3 and len(bwd_f) == 2
     B.assert_rejects(fwd_f, *ref['fwd'], B.OUT_REL_BF16, c=B.C_PAINT)
     B.assert_rejects(bwd_f, *ref['bwd'], B.OUT_REL_F32, c=B.C_PAINT)
+
+
+# ------------------------------------------------------------------------------------------------ head and elementwise
+def _emulated_focal(x, t, w, gamma, alpha, scale):
+    """csrc/head.cu's focal element in fp32: p = 1 / (1 + exp(-x)), 1 - p in fp32, the clamp to FLT_MIN."""
+    xf = x.float()
+    p = 1 / (1 + torch.exp(-xf))
+    q = 1 - p
+    pos = t.view(-1, 1) == torch.arange(x.shape[1]).view(1, -1)
+    lp, lq = torch.log(p.clamp(min=B.FLT_MIN)), torch.log(q.clamp(min=B.FLT_MIN))
+    pg, qg = p ** gamma, q ** gamma
+    l = torch.where(pos, -alpha * qg * lp, -(1 - alpha) * pg * lq) * w.view(-1, 1)
+    g = torch.where(pos, -alpha * qg * (q - gamma * p * lp), -(1 - alpha) * pg * (gamma * q * lq - p))
+    return l, g * scale * w.view(-1, 1)
+
+
+def test_bound_accepts_emulated_focal_and_rejects_its_faults():
+    gen = torch.Generator().manual_seed(6)
+    n, C = 300, 284
+    x, t, w = B.focal_operands(n, C, gen)
+    x = x.bfloat16()
+    l, g = _emulated_focal(x, t, w, 2.0, 0.25, 0.37)
+    ref = B.focal_ref(x, t, w, 2.0, 0.25, 0.37)
+    n_blocks = (n * C + 255) // 256
+    total, A = B.focal_sum_bound(ref, n_blocks)
+    out = l.sum()
+    B.assert_within(out, total, A, 1, B.OUT_REL_F32, 'emulated focal sum')
+    B.assert_rejects(B.focal_faults_fwd(x, t, w, 2.0, 0.25, out), total, A, 1, B.OUT_REL_F32)
+    gb = g.bfloat16()
+    Ag = ref['K'] * ref['g'].abs()
+    B.assert_within(gb, ref['g'], Ag, B.FOCAL_ELEM, B.OUT_REL_BF16, 'emulated focal grad')
+    B.assert_rejects(B.focal_faults_bwd(x, t, w, 2.0, 0.25, 0.37, gb), ref['g'], Ag, B.FOCAL_ELEM, B.OUT_REL_BF16)
+    xw = B.focal_operands(n, C, gen, wide=True)[0].bfloat16()      # the wide range: elementwise bound and faults
+    gw = _emulated_focal(xw, t, w, 2.0, 0.25, 0.37)[1].bfloat16()
+    ref = B.focal_ref(xw, t, w, 2.0, 0.25, 0.37)
+    Ag = ref['K'] * ref['g'].abs()
+    B.assert_within(gw, ref['g'], Ag, B.FOCAL_ELEM, B.OUT_REL_BF16, 'emulated focal grad, wide logits')
+    B.assert_rejects(B.focal_faults_bwd(xw, t, w, 2.0, 0.25, 0.37, gw), ref['g'], Ag, B.FOCAL_ELEM, B.OUT_REL_BF16)
+
+
+def test_bound_accepts_emulated_bias_act_and_act_bwd():
+    gen = torch.Generator().manual_seed(7)
+    rows, C = 301, 16
+    for act in (0, 1, 2):
+        x = torch.randn(rows, C, generator=gen).bfloat16()
+        b = torch.randn(C, generator=gen)
+        r = torch.randn(rows, C, generator=gen).bfloat16()
+        z = x.float() + b + r.float()
+        y = B._act(z, act).bfloat16()
+        ref, A, n_red = B.bias_act_ref(x, b, r, act)
+        B.assert_within(y, ref, A, n_red, B.OUT_REL_BF16, f'emulated bias act {act}')
+        B.assert_rejects(B.bias_act_faults(y, x, b, r, act, 256 * 8 // C), ref, A, n_red, B.OUT_REL_BF16)
+        dy = torch.randn(rows * C, generator=gen).bfloat16()
+        zf = z.reshape(-1)
+        yf = y.reshape(-1)
+        d = torch.ones_like(zf) if act == 0 else ((yf > 0).float() if act == 1 else torch.where(yf > 0, 1.0, yf.float() + 1))
+        dx = (dy.float() * d).bfloat16()
+        ref, A, n_red, fixed = B.act_bwd_ref(dy, zf, yf, act)
+        B.assert_within(dx[:-3], ref[:-3], A[:-3], n_red, B.OUT_REL_BF16, f'emulated act bwd {act}', fixed=fixed[:-3])
+        B.assert_rejects(B.act_bwd_faults(dx[:-3], dy[:-3], zf[:-3], act), ref[:-3], A[:-3], n_red, B.OUT_REL_BF16,
+                         fixed[:-3])
+
+
+def test_bound_accepts_emulated_interpolation_and_rejects_its_faults():
+    import numpy as np
+    g = np.random.RandomState(8)
+    ts, C = 2, 18
+    c = np.unique(np.concatenate([g.randint(0, 2, (600, 1)), g.randint(-6, 6, (600, 3)) * ts], 1), axis=0)
+    feats = torch.from_numpy(g.randn(c.shape[0], C)).float().bfloat16()
+    q = np.concatenate([g.randint(0, 2, (500, 1)), g.randint(-13, 13, (500, 3))], 1)
+    ref, A, n_red, rows, wt = B.interp_ref(c, feats, ts, q)
+    f = feats.float()
+    out = (f[rows.clamp(min=0)] * (rows >= 0)[..., None] * wt.float()[..., None]).sum(1)
+    B.assert_within(out, ref, A, n_red, B.OUT_REL_F32, 'emulated interpolation')
+    assert bool((rows < 0).any() & (rows >= 0).any()) and bool((np.asarray(q)[:, 1:] < 0).any())
+    B.assert_rejects(B.interp_faults(out, c, feats, ts, q), ref, A, n_red, B.OUT_REL_F32)

@@ -707,10 +707,10 @@ def _step(model, batch):
     sum(losses.values()).backward()
 
 
-def _census_model(variant):
-    """One bf16 training forward + backward of `variant` under the profiler (in the child). C3 / C4 keep the published
-    channel widths (which, with the strides, decide every instance: conv_tma_run, conv_wgrad_any, _ConvBlock2D) on one
-    or two scans of two small views."""
+def census_step(variant):
+    """(model, batch) of the census step of `variant` in bf16 training mode. C3 / C4 keep the published channel widths
+    (which, with the strides, decide every instance: conv_tma_run, conv_wgrad_any, _ConvBlock2D) on one or two scans of
+    two small views. Shared with the whole-library census of test_head_elementwise_bf16_gpu.py."""
     import warnings
     from embodiedscan_b200 import MODELS
     from embodiedscan_b200 import synth as SY
@@ -731,6 +731,12 @@ def _census_model(variant):
     with warnings.catch_warnings():
         warnings.simplefilter('ignore')
         model = MODELS.build(dict(cfg, compute_dtype=BF)).to(DEV).train()
+    return model, batch
+
+
+def _census_model(variant):
+    """One bf16 training forward + backward of `variant` under the profiler (in the child)."""
+    model, batch = census_step(variant)
     return _instances(lambda: _step(model, batch))[1]
 
 

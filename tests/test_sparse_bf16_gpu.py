@@ -231,22 +231,35 @@ def _norm_case(sizes, C, res_too, gen):
     return x, dy, res, gamma, beta
 
 
-def _check_norm(x, dy, res, gamma, beta, y, xg, sizes, eps, pivot, what):
+def _check_norm(x, dy, res, gamma, beta, y, xg, sizes, eps, pivot, what, act=1):
+    """Forward: ReLU and ELU are 1-Lipschitz, so the bound on z carries over to y. Backward, ReLU: the derivative read
+    from the kernel's own y (a step: it must be the kernel's). ELU: the derivative e^z at the float64 z, and the kernel's
+    y + 1 is off by at most the forward bound of y, which, times |dy|, is a `fixed` term carried through the backward
+    formula (bf16_bounds.seg_norm_bwd_fixed)."""
     z, A, n_red, st = B.seg_norm_ref(x, sizes, gamma.detach(), beta.detach(), eps, res, pivot)
-    r = B.assert_within(y, z.clamp(min=0), A, n_red, B.OUT_REL_BF16, f'{what} fwd')   # ReLU is 1-Lipschitz
-    gy = dy.double() * (y > 0)
+    ya = B._act(z, act)
+    r = B.assert_within(y, ya, A, n_red, B.OUT_REL_BF16, f'{what} fwd')
+    F_dx = F_dg = F_db = 0.0
+    if act == 1:
+        gy = dy.double() * (y > 0)
+    else:
+        gy = dy.double() * torch.where(z > 0, 1.0, torch.exp(z))
+        y_err = (B.OUT_REL_BF16 * ya.abs() + B.C_ACC * B.U32 * n_red * A) * (1 + 2.0 ** -7)
+        F_dx, F_dg, F_db = B.seg_norm_bwd_fixed(x, dy.double().abs() * y_err, st)
+        F_dx = F_dx * gamma.detach().double().abs().view(1, -1)
     (dx, A_dx), (dg, A_dg), (db, A_db) = B.seg_norm_bwd_ref(x, gy, gamma.detach(), st)
     N = float(x.shape[0])
-    r = max(r, B.assert_within(xg, dx, A_dx, n_red, B.OUT_REL_BF16, f'{what} dx'))
-    r = max(r, B.assert_within(gamma.grad.view(-1), dg, A_dg, N, B.OUT_REL_F32, f'{what} dgamma'))
-    r = max(r, B.assert_within(beta.grad.view(-1), db, A_db, N, B.OUT_REL_F32, f'{what} dbeta'))
+    r = max(r, B.assert_within(xg, dx, A_dx, n_red, B.OUT_REL_BF16, f'{what} dx', fixed=F_dx))
+    r = max(r, B.assert_within(gamma.grad.view(-1), dg, A_dg, N, B.OUT_REL_F32, f'{what} dgamma', fixed=F_dg))
+    r = max(r, B.assert_within(beta.grad.view(-1), db, A_db, N, B.OUT_REL_F32, f'{what} dbeta', fixed=F_db))
     return r
 
 
+@pytest.mark.parametrize('act', [1, 2], ids=['relu', 'elu'])
 @pytest.mark.parametrize('C', [64, 12])
-def test_instance_norm_bf16(C):
-    """MinkowskiInstanceNorm + ReLU in bf16 (esb_norm_fwd / esb_norm_bwd with one segment per scan): 4 scans of unequal size,
-    one spanning three 256-row statistics blocks. C = 12 takes the non-vec8 apply kernels."""
+def test_instance_norm_bf16(C, act):
+    """MinkowskiInstanceNorm + ReLU / ELU in bf16 (esb_norm_fwd / esb_norm_bwd with one segment per scan): 4 scans of
+    unequal size, one spanning three 256-row statistics blocks. C = 12 takes the non-vec8 apply kernels."""
     from embodiedscan_b200 import sparse as SP
     gen = torch.Generator().manual_seed(C)
     sizes = [700, 37, 258, 129]
@@ -256,18 +269,19 @@ def test_instance_norm_bf16(C):
     xg = x.clone().requires_grad_(True)
 
     def run():
-        y = SP.seg_norm(xg, gamma, beta, seg_off, row_seg, 4, max(sizes), 1e-8, SP.ACT_RELU)
+        y = SP.seg_norm(xg, gamma, beta, seg_off, row_seg, 4, max(sizes), 1e-8, act)
         y.backward(dy)
         return y
     y, seen = _instances(run)
-    _claim(seen, NORM_STATS + (NORM_VEC8 if C % 8 == 0 else NORM_SCALAR), f'instance norm C {C}')
-    r = _check_norm(x, dy, None, gamma, beta, y.detach(), xg.grad, sizes, 1e-8, False, 'instance norm')
+    _claim(seen, NORM_STATS + (NORM_VEC8 if C % 8 == 0 else NORM_SCALAR), f'instance norm C {C} act {act}')
+    r = _check_norm(x, dy, None, gamma, beta, y.detach(), xg.grad, sizes, 1e-8, False, 'instance norm', act)
     print(f'ratio {r:.4g}')
 
 
+@pytest.mark.parametrize('act', [1, 2], ids=['relu', 'elu'])
 @pytest.mark.parametrize('C,N', [(8, 3001), (2048, 517), (12, 1001)])
-def test_batch_norm_bf16(C, N):
-    """BatchNorm + residual + ReLU in bf16 on the training path: the fused single-pass kernels at their shared-memory edges
+def test_batch_norm_bf16(C, N, act):
+    """BatchNorm + residual + ReLU / ELU in bf16 on the training path: the fused single-pass kernels at their shared-memory edges
     C = 8 (256 rows per step) and C = 2048 (one row per step), and the esb_norm_fwd fallback at C = 12 (not a multiple of 8).
     Backward through esb_norm_bwd. The pivot row is offset from the mean to exercise the shifted statistics."""
     from embodiedscan_b200 import sparse as SP
@@ -282,13 +296,14 @@ def test_batch_norm_bf16(C, N):
     xg = x.clone().requires_grad_(True)
 
     def run():
-        y = SP.batch_norm_rows(xg, bn, True, SP.ACT_RELU, res)
+        y = SP.batch_norm_rows(xg, bn, True, act, res)
         y.backward(dy)
         return y
     y, seen = _instances(run)
     fused = C % 8 == 0
-    _claim(seen, BN_FUSED + [NORM_STATS[-1], NORM_VEC8[1]] if fused else NORM_STATS + NORM_SCALAR, f'batch norm C {C}')
-    r = _check_norm(x, dy, res, bn.weight, bn.bias, y.detach(), xg.grad, [N], bn.eps, fused, 'batch norm')
+    _claim(seen, BN_FUSED + [NORM_STATS[-1], NORM_VEC8[1]] if fused else NORM_STATS + NORM_SCALAR,
+           f'batch norm C {C} act {act}')
+    r = _check_norm(x, dy, res, bn.weight, bn.bias, y.detach(), xg.grad, [N], bn.eps, fused, 'batch norm', act)
     print(f'ratio {r:.4g}')
 
 
