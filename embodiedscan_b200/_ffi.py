@@ -29,9 +29,11 @@ SIGNATURES = {
     'esb_generative_children': ('pqipp', 'i'),
     'esb_spconv_fwd': ('ppppqiiiiip', 'i'),
     'esb_spconv_wgrad': ('ppppppqiiiip', 'i'),
+    'esb_spconv_wgrad_slot': ('ppppppqiiiip', 'i'),
     'esb_kmap_tile_masks': ('piqpp', 'i'),
     'esb_spconv_tc_fwd': ('pppppqiiiip', 'i'),
     'esb_spconv_tc_wgrad': ('ppppppqiiip', 'i'),
+    'esb_spconv_tc_wgrad_slot': ('ppppppqiiip', 'i'),
     'esb_maxpool_fwd': ('ppppqiiip', 'i'),
     'esb_maxpool_bwd': ('pppqiip', 'i'),
     'esb_norm_fwd': ('ppppiqiippfppfipppip', 'i'),
@@ -87,11 +89,12 @@ _lib = None
 KERNELS_PER_CALL = {
     'esb_voxelize_points': 1, 'esb_coord_unique': 6, 'esb_hash_build': 2, 'esb_hash_lookup': 1, 'esb_kernel_map': 1,
     'esb_kernel_map_transpose': 2, 'esb_kmap_pairs': 3, 'esb_generative_children': 1, 'esb_spconv_fwd': 1,
-    'esb_spconv_wgrad': 1, 'esb_maxpool_fwd': 1, 'esb_maxpool_bwd': 1, 'esb_norm_fwd': 5, 'esb_norm_apply': 1,
+    'esb_spconv_wgrad': 1, 'esb_spconv_wgrad_slot': 1, 'esb_maxpool_fwd': 1, 'esb_maxpool_bwd': 1, 'esb_norm_fwd': 5, 'esb_norm_apply': 1,
     'esb_norm_bwd': 2, 'esb_batchnorm_fwd_fused': 2, 'esb_paint_fwd': 1, 'esb_paint_bwd': 1, 'esb_fcaf3d_targets': 5,
     'esb_focal_loss_fwd': 1, 'esb_focal_loss_bwd': 1, 'esb_nms_bev_segmented': 1, 'esb_iou_bev_pairwise': 1,
     'esb_img_normalize': 1, 'esb_unproject_depth': 3, 'esb_grad_clip_coef': 2, 'esb_adamw_step_groups': 1,
-    'esb_cast_f32_to_bf16': 1, 'esb_spconv_tc_fwd': 1, 'esb_spconv_tc_wgrad': 1, 'esb_kmap_tile_masks': 1,
+    'esb_cast_f32_to_bf16': 1, 'esb_spconv_tc_fwd': 1, 'esb_spconv_tc_wgrad': 1, 'esb_spconv_tc_wgrad_slot': 1,
+    'esb_kmap_tile_masks': 1,
     'esb_chamfer_fwd': 2, 'esb_chamfer_bwd': 4, 'esb_nms3d_9dof': 2,
 }
 launch_counter = {'kernels': 0, 'calls': 0, 'by_name': {}}

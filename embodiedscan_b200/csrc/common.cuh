@@ -45,7 +45,9 @@ static inline size_t esb_align(size_t x, size_t a = 256) { return (x + a - 1) / 
 // in index order. The scratch comes from the device's stream-ordered pool and is released on the same stream.
 cudaError_t esb_scratch_alloc(void** p, size_t bytes, cudaStream_t s);
 cudaError_t esb_scratch_free(void* p, cudaStream_t s);
-// out[j] (+)= sum over p = 0 .. n_parts-1 of part[p * width + j], in that order (accumulate = 0 overwrites out)
+// out[j] (+)= sum over p = 0 .. n_parts-1 of part[p * width + j], in that order. accumulate = 0 overwrites out; 1 starts the
+// add chain from out[j]; 2 finishes the sum from +0 and adds it to out[j] with one rounded add (gradient slots, see
+// esb_norm_bwd: the slot then receives exactly what autograd's `grad += fresh` would add)
 int esb_sum_partial_rows(const float* part, int n_parts, long long width, float* out, int accumulate, cudaStream_t s);
 
 // streaming multiprocessors of the current device (grid sizing; read once per device)

@@ -46,7 +46,8 @@ __device__ __forceinline__ float add_chain_contiguous(const float* __restrict__ 
 // callers have few columns and many parts (a loss sum has one column and thousands of parts), so the whole block loads:
 // tiles of kSumTile / cw parts x cw columns, every thread kSumLoads independent coalesced loads, through shared memory to
 // thread c, which adds its column in part order, each add rounded on its own. The next tile is in flight in the loaders'
-// registers while the current one is added.
+// registers while the current one is added. accumulate: 0 = out[j] = the sum from +0; 1 = the chain starts from out[j];
+// 2 = out[j] + the finished sum from +0, one rounded add (how a gradient slot receives one backward pass's sum).
 __global__ void __launch_bounds__(kSumThreads) sum_partial_rows_kernel(const float* __restrict__ part, int n_parts,
                                                                        long long width, float* __restrict__ out,
                                                                        int accumulate, int cw) {
@@ -65,7 +66,7 @@ __global__ void __launch_bounds__(kSumThreads) sum_partial_rows_kernel(const flo
       v[k] = col_ok && p < n_parts ? part[(long long)p * width + j] : 0.f;
     }
   };
-  float s = adder && accumulate ? out[j] : 0.f;
+  float s = adder && accumulate == 1 ? out[j] : 0.f;
   if (n_parts > 0) load(0);
   for (int p0 = 0; p0 < n_parts; p0 += rows) {
     __syncthreads();                                  // the adders are done with the previous tile
@@ -95,7 +96,7 @@ __global__ void __launch_bounds__(kSumThreads) sum_partial_rows_kernel(const flo
       for (int u = 0; r + u < n; ++u) s = __fadd_rn(s, col[(r + u) * cw]);
     }
   }
-  if (adder) out[j] = s;
+  if (adder) out[j] = accumulate == 2 ? __fadd_rn(out[j], s) : s;
 }
 
 }  // namespace

@@ -211,11 +211,10 @@ extern "C" int esb_spconv_fwd(const void* x, const void* w, const int* nbr, void
   return ESB_OK;
 }
 
-// dw (K,cin,cout) fp32 += the weight gradient (zeroed by the caller for a plain gradient); the pair splits' partials are
-// added in split order.
-extern "C" int esb_spconv_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out,
-                                const int* k_offsets, float* dw, long long n_pairs_hint, int cin, int cout, int K,
-                                int dtype, void* stream_) {
+namespace {
+// accumulate: esb_sum_partial_rows' mode for dw (1: the chain starts from dw; 2: dw + the finished sum)
+int spconv_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out, const int* k_offsets, float* dw,
+                 long long n_pairs_hint, int cin, int cout, int K, int dtype, int accumulate, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   ESB_CHECK_ARG(cin > 0 && cout > 0 && K > 0, "esb_spconv_wgrad: bad channel/kernel sizes");
   ESB_CHECK_ARG(dtype == ESB_F32 || dtype == ESB_BF16, "esb_spconv_wgrad: dtype must be f32 or bf16");
@@ -239,7 +238,24 @@ extern "C" int esb_spconv_wgrad(const void* x, const void* dy, const int* pair_i
     spconv_wgrad_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)dy,
                                                                   pair_in, pair_out, k_offsets, part, cin, cout, splits);
   ESB_CUDA_LAUNCH_CHECK("spconv_wgrad_kernel");
-  int rc = esb_sum_partial_rows(part, splits, width, dw, 1, stream);
+  int rc = esb_sum_partial_rows(part, splits, width, dw, accumulate, stream);
   ESB_CUDA_CALL(esb_scratch_free(part, stream));
   return rc;
+}
+}  // namespace
+
+// dw (K,cin,cout) fp32 += the weight gradient (zeroed by the caller for a plain gradient); the pair splits' partials are
+// added in split order, starting from dw.
+extern "C" int esb_spconv_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out,
+                                const int* k_offsets, float* dw, long long n_pairs_hint, int cin, int cout, int K,
+                                int dtype, void* stream) {
+  return spconv_wgrad(x, dy, pair_in, pair_out, k_offsets, dw, n_pairs_hint, cin, cout, K, dtype, 1, stream);
+}
+
+// The same into a gradient slot that may hold earlier backward passes: the splits are added in split order from +0 and
+// dw = dw + that sum, one rounded add per element (on a zeroed dw: the bits of esb_spconv_wgrad).
+extern "C" int esb_spconv_wgrad_slot(const void* x, const void* dy, const int* pair_in, const int* pair_out,
+                                     const int* k_offsets, float* dw, long long n_pairs_hint, int cin, int cout, int K,
+                                     int dtype, void* stream) {
+  return spconv_wgrad(x, dy, pair_in, pair_out, k_offsets, dw, n_pairs_hint, cin, cout, K, dtype, 2, stream);
 }

@@ -347,10 +347,12 @@ spconv_tc_wgrad_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16*
 }
 
 // dw[k] += the partials of the chunks of offset k, in chunk order (chunks enumerate offset by offset, as in the kernel above).
+// slot = 0: the add chain starts from dw[k]. slot = 1 (gradient slots): the chunks are added from +0 and the finished sum is
+// added to dw[k] with one rounded add, as autograd's `grad += fresh`.
 // Thread = 4 consecutive columns of one offset (cin * cout is a multiple of 4096; the scratch partials are 16-byte aligned):
 // the 16-byte loads of 8 chunks are in flight before their in-order adds, one add chain per column.
 __global__ void spconv_wgrad_reduce_kernel(const float* __restrict__ part, const int* __restrict__ k_offsets, float* __restrict__ dw,
-                                           int cin, int cout, int K, int chunk_pairs) {
+                                           int cin, int cout, int K, int chunk_pairs, int slot) {
   constexpr int D = 8;
   const long long e = (blockIdx.x * (long long)blockDim.x + threadIdx.x) * 4;
   const long long per_k = (long long)cin * cout;
@@ -360,7 +362,11 @@ __global__ void spconv_wgrad_reduce_kernel(const float* __restrict__ part, const
   int c0 = 0;
   for (int kk = 0; kk < k; ++kk) c0 += (k_offsets[kk + 1] - k_offsets[kk] + chunk_pairs - 1) / chunk_pairs;
   const int nch = (k_offsets[k + 1] - k_offsets[k] + chunk_pairs - 1) / chunk_pairs;
-  float s[4] = {dw[e], dw[e + 1], dw[e + 2], dw[e + 3]};
+  float s[4] = {0.f, 0.f, 0.f, 0.f};
+  if (!slot) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) s[q] = dw[e + q];
+  }
   const float4* src = reinterpret_cast<const float4*>(part + (long long)c0 * per_k + j);
   const long long stride = per_k / 4;
   for (int c = 0; c < nch; c += D) {
@@ -378,7 +384,7 @@ __global__ void spconv_wgrad_reduce_kernel(const float* __restrict__ part, const
       }
   }
 #pragma unroll
-  for (int q = 0; q < 4; ++q) dw[e + q] = s[q];
+  for (int q = 0; q < 4; ++q) dw[e + q] = slot ? __fadd_rn(dw[e + q], s[q]) : s[q];
 }
 
 template <int N_TILE, int STAGES, bool B_MN>
@@ -463,11 +469,9 @@ extern "C" int esb_spconv_tc_fwd(const void* x, const void* wt, const int* nbr, 
   return ESB_OK;
 }
 
-// bf16 tensor-core wgrad over pair lists; dw (K,cin,cout) fp32 += the weight gradient (zeroed by the caller for a plain
-// gradient). The pair chunks of an offset are added in chunk order: the result does not depend on scheduling.
-extern "C" int esb_spconv_tc_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out,
-                                   const int* k_offsets, float* dw, long long n_pairs_hint, int cin, int cout, int K,
-                                   void* stream_) {
+namespace {
+int spconv_tc_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out, const int* k_offsets, float* dw,
+                    long long n_pairs_hint, int cin, int cout, int K, int slot, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   ESB_CHECK_ARG(cin % 64 == 0 && cout % 64 == 0 && cin > 0 && cout > 0, "esb_spconv_tc_wgrad: channels must be multiples of 64");
   int n_tile = (cout % 128 == 0) ? 128 : 64;
@@ -487,10 +491,28 @@ extern "C" int esb_spconv_tc_wgrad(const void* x, const void* dy, const int* pai
                : launch_wgrad<64, 4>(x, dy, pair_in, pair_out, k_offsets, part, cin, cout, K, n_chunks, chunk_pairs, stream);
   if (rc == ESB_OK) {
     spconv_wgrad_reduce_kernel<<<esb_div_up((long long)K * cin * cout / 4, 256), 256, 0, stream>>>(part, k_offsets, dw, cin, cout,
-                                                                                                 K, chunk_pairs);
+                                                                                                 K, chunk_pairs, slot);
   }
   ESB_CUDA_CALL(esb_scratch_free(part, stream));
   if (rc != ESB_OK) return rc;
   ESB_CUDA_LAUNCH_CHECK("spconv_tc_wgrad_kernel");
   return ESB_OK;
+}
+}  // namespace
+
+// bf16 tensor-core wgrad over pair lists; dw (K,cin,cout) fp32 += the weight gradient (zeroed by the caller for a plain
+// gradient). The pair chunks of an offset are added in chunk order, starting from dw: the result does not depend on
+// scheduling.
+extern "C" int esb_spconv_tc_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out,
+                                   const int* k_offsets, float* dw, long long n_pairs_hint, int cin, int cout, int K,
+                                   void* stream) {
+  return spconv_tc_wgrad(x, dy, pair_in, pair_out, k_offsets, dw, n_pairs_hint, cin, cout, K, 0, stream);
+}
+
+// The same into a gradient slot that may hold earlier backward passes: the chunks are added in chunk order from +0 and
+// dw = dw + that sum, one rounded add per element (on a zeroed dw: the bits of esb_spconv_tc_wgrad).
+extern "C" int esb_spconv_tc_wgrad_slot(const void* x, const void* dy, const int* pair_in, const int* pair_out,
+                                        const int* k_offsets, float* dw, long long n_pairs_hint, int cin, int cout, int K,
+                                        void* stream) {
+  return spconv_tc_wgrad(x, dy, pair_in, pair_out, k_offsets, dw, n_pairs_hint, cin, cout, K, 1, stream);
 }

@@ -199,7 +199,8 @@ __global__ void norm_bwd_apply_vec8_kernel(const T* __restrict__ x, const T* __r
                                            const float* __restrict__ mean, const float* __restrict__ rstd,
                                            const float* __restrict__ gamma, const float* __restrict__ sg,
                                            const float* __restrict__ sgx, T* __restrict__ dx, T* __restrict__ dres,
-                                           long long N, long long n_vec, int C, int act) {
+                                           long long N, long long n_vec, int C, int act, float* __restrict__ slot_g,
+                                           float* __restrict__ slot_gx) {
   long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (t >= n_vec) return;
   const int cv = C >> 3;
@@ -222,6 +223,13 @@ __global__ void norm_bwd_apply_vec8_kernel(const T* __restrict__ x, const T* __r
   }
   store8<T>(dx + t * 8, ov);
   if (dres) store8<T>(dres + t * 8, gv);
+  if (slot_g != nullptr && r == 0) {          // one segment: row 0's threads own the columns of the gradient slots
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      slot_g[c0 + i] = __fadd_rn(slot_g[c0 + i], sg[c0 + i]);
+      slot_gx[c0 + i] = __fadd_rn(slot_gx[c0 + i], sgx[c0 + i]);
+    }
+  }
 }
 
 // backward reduce: sg[s][c] = sum g ; sgx[s][c] = sum g * xhat, with g = dy * act'(y); partials per row block as above
@@ -262,14 +270,16 @@ __global__ void norm_bwd_reduce_kernel(const T* __restrict__ x, const T* __restr
   }
 }
 
-// dx = gamma*rstd*(g - mean_s(g) - xhat*mean_s(g*xhat)) ; dres = g
+// dx = gamma*rstd*(g - mean_s(g) - xhat*mean_s(g*xhat)) ; dres = g ; with slots (one segment): slot_g[c] += sg[c] and
+// slot_gx[c] += sgx[c], one rounded add each, by the threads of row 0
 template <typename T>
 __global__ void norm_bwd_apply_kernel(const T* __restrict__ x, const T* __restrict__ y, const T* __restrict__ dy,
                                       const int* __restrict__ row_seg, const int* __restrict__ seg_off,
                                       const float* __restrict__ mean, const float* __restrict__ rstd,
                                       const float* __restrict__ gamma, const float* __restrict__ sg,
                                       const float* __restrict__ sgx, T* __restrict__ dx, T* __restrict__ dres,
-                                      long long N, int C, int act) {
+                                      long long N, int C, int act, float* __restrict__ slot_g,
+                                      float* __restrict__ slot_gx) {
   long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (t >= N * C) return;
   long long r = t / C;
@@ -283,6 +293,10 @@ __global__ void norm_bwd_apply_kernel(const T* __restrict__ x, const T* __restri
   float v = gm * rs * (g - sg[s * C + c] * inv_n - xh * sgx[s * C + c] * inv_n);
   dx[t] = esb_from_float<T>(v);
   if (dres) dres[t] = esb_from_float<T>(g);
+  if (slot_g != nullptr && r == 0) {
+    slot_g[c] = __fadd_rn(slot_g[c], sg[c]);
+    slot_gx[c] = __fadd_rn(slot_gx[c], sgx[c]);
+  }
 }
 
 // y = act(x + bias[c] + res) over (rows, C) row-major (an NHWC activation is exactly that), 8 channels per thread.
@@ -546,7 +560,11 @@ extern "C" int esb_norm_bwd(const void* x, const void* y, const void* dy, const 
                             const float* gamma, int act, float* sg, float* sgx, void* dx, void* dres, int zero_sums,
                             int dtype, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  // zero_sums = 0: sg/sgx are the (already zeroed, used once per step) gradient slots of beta/gamma in the flat arena
+  // zero_sums = 0: sg/sgx are the gradient slots of beta/gamma in the flat arena (one segment). They may hold the gradients
+  // of earlier backward passes (micro-batches accumulated without zero_grad), so this pass's column sums are finished in
+  // scratch from +0, dx is computed from them alone, and the apply kernel adds them to the slots with one rounded add each:
+  // slot + sum, what autograd's `grad += fresh` computes. On a zeroed slot that is the sum itself, bit for bit.
+  ESB_CHECK_ARG(zero_sums || S == 1, "esb_norm_bwd: gradient slots (zero_sums = 0) take one segment");
   if (zero_sums) {
     ESB_CUDA_CALL(cudaMemsetAsync(sg, 0, sizeof(float) * S * C, stream));
     ESB_CUDA_CALL(cudaMemsetAsync(sgx, 0, sizeof(float) * S * C, stream));
@@ -556,20 +574,27 @@ extern "C" int esb_norm_bwd(const void* x, const void* y, const void* dy, const 
   dim3 grid(esb_div_up(max_seg_rows > 0 ? max_seg_rows : 1, rpb), S, esb_div_up(C, 32)), block(32, 8);
   const long long width = (long long)S * C;
   float* part = nullptr;
-  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, sizeof(float) * 2 * grid.x * width, stream));
+  ESB_CUDA_CALL(esb_scratch_alloc((void**)&part, sizeof(float) * 2 * (grid.x + (zero_sums ? 0 : 1)) * width, stream));
+  float* slot_g = zero_sums ? nullptr : sg;
+  float* slot_gx = zero_sums ? nullptr : sgx;
+  if (!zero_sums) {
+    sg = part + 2 * grid.x * width;
+    sgx = sg + width;
+  }
   int rc = ESB_OK;
   DISPATCH_T(dtype, {
     norm_bwd_reduce_kernel<T><<<grid, block, 0, stream>>>((const T*)x, (const T*)y, (const T*)dy, seg_off, mean, rstd,
                                                           part, part + grid.x * width, C, rpb, act, (int)N);
-    rc = esb_sum_partial_rows(part, (int)grid.x, width, sg, 1, stream);
-    if (rc == ESB_OK) rc = esb_sum_partial_rows(part + grid.x * width, (int)grid.x, width, sgx, 1, stream);
+    rc = esb_sum_partial_rows(part, (int)grid.x, width, sg, 0, stream);
+    if (rc == ESB_OK) rc = esb_sum_partial_rows(part + grid.x * width, (int)grid.x, width, sgx, 0, stream);
     if (C % 8 == 0)
       norm_bwd_apply_vec8_kernel<T><<<esb_div_up(N * (C / 8), 256), 256, 0, stream>>>(
           (const T*)x, (const T*)y, (const T*)dy, row_seg, seg_off, mean, rstd, gamma, sg, sgx, (T*)dx, (T*)dres, N,
-          N * (C / 8), C, act);
+          N * (C / 8), C, act, slot_g, slot_gx);
     else
       norm_bwd_apply_kernel<T><<<esb_div_up(N * C, 256), 256, 0, stream>>>(
-          (const T*)x, (const T*)y, (const T*)dy, row_seg, seg_off, mean, rstd, gamma, sg, sgx, (T*)dx, (T*)dres, N, C, act);
+          (const T*)x, (const T*)y, (const T*)dy, row_seg, seg_off, mean, rstd, gamma, sg, sgx, (T*)dx, (T*)dres, N, C, act,
+          slot_g, slot_gx);
   });
   ESB_CUDA_CALL(esb_scratch_free(part, stream));
   if (rc != ESB_OK) return rc;

@@ -159,8 +159,10 @@ class MultiModal3DModel(nn.Module):
 
     # ---- mmengine BaseModel contract (†upstream) -------------------------------------------------------------
     def train_step(self, data, optim_wrapper):
-        data = self.data_preprocessor(data, True)
-        loss, log_vars = parse_losses(self(**data, mode='loss'))
+        with optim_wrapper.optim_context(self):
+            data = self.data_preprocessor(data, True)
+            losses = self(**data, mode='loss')
+        loss, log_vars = parse_losses(losses)
         optim_wrapper.update_params(loss)
         return detach_log_vars(log_vars)
 

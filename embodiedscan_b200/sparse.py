@@ -41,20 +41,33 @@ def _timed_conv_call(kind, kmap, cin, cout, dtype, *args):
 
 
 def _count_use(*params):
-    """Forward side of the 'direct' gradient path: a parameter used n times in one step gets its hooks fired after the
-    n-th backward contribution (what autograd's AccumulateGrad does for ordinary parameters)."""
+    """Forward side of the 'direct' gradient path: counts the uses of an arena parameter in one forward pass
+    (`_esb_uses` = backward contributions still to come, `_esb_pass_uses` = uses of this pass)."""
     for p in params:
         if p is not None and getattr(p, '_esb_grad_direct', False):
             p._esb_uses = getattr(p, '_esb_uses', 0) + 1
+            p._esb_pass_uses = getattr(p, '_esb_pass_uses', 0) + 1
 
 
-def _fire_grad_hooks(*params):
-    for p in params:
-        left = getattr(p, '_esb_uses', 1) - 1
-        p._esb_uses = max(left, 0)
-        if left <= 0:
+def _direct(p) -> bool:
+    """Whether a kernel may add this backward's gradient of `p` straight into its arena slot: only for a parameter used
+    once in the pass. A slot must receive one pass's gradient with ONE rounded add (slot + sum, as autograd's
+    AccumulateGrad adds the sum of a leaf's contributions), so that micro-batches accumulate bit for bit as on plain
+    autograd; a parameter used n times returns its gradients to autograd, which sums them before that one add."""
+    return (getattr(p, '_esb_grad_direct', False) and p.grad is not None
+            and getattr(p, '_esb_pass_uses', 0) == 1)
+
+
+def _release_use(p, direct: bool):
+    """Backward side: after the last contribution of the pass the use counts restart, and a direct parameter fires its
+    hooks (what autograd's AccumulateGrad fires for the others: the bucket all-reduce bookkeeping)."""
+    left = getattr(p, '_esb_uses', 1) - 1
+    p._esb_uses = max(left, 0)
+    if left <= 0:
+        p._esb_pass_uses = 0
+        if direct:
             for hook in (getattr(p, '_post_accumulate_grad_hooks', None) or {}).values():
-                hook(p)       # what autograd's AccumulateGrad would have fired (bucket all-reduce bookkeeping)
+                hook(p)
 
 
 def _offsets(kernel_size: int, scale: int) -> List[int]:
@@ -311,20 +324,19 @@ class _SparseConv(torch.autograd.Function):
         if ctx.needs_input_grad[1]:
             pin, pout, koff, tot = kmap.pairs
             weight = ctx.weight
-            direct = getattr(weight, '_esb_grad_direct', False) and weight.grad is not None
-            # arena parameters: the kernel accumulates straight into the flat gradient buffer (no zeros + add_ pass)
+            direct = _direct(weight)
+            # arena parameters: the kernel adds its finished sum straight into the flat gradient buffer (no zeros + add_ pass)
             dw = weight.grad if direct else torch.zeros((kmap.K, cin, cout), dtype=torch.float32, device=x.device)
+            slot = '_slot' if direct else ''
             if ctx.tc:
-                _timed_conv_call('wgrad', kmap, cin, cout, x.dtype, 'esb_spconv_tc_wgrad', ptr(x), ptr(dy), ptr(pin),
-                                 ptr(pout), ptr(koff), ptr(dw), tot, cin, cout, kmap.K, stream())
+                _timed_conv_call('wgrad', kmap, cin, cout, x.dtype, 'esb_spconv_tc_wgrad' + slot, ptr(x), ptr(dy),
+                                 ptr(pin), ptr(pout), ptr(koff), ptr(dw), tot, cin, cout, kmap.K, stream())
             else:
-                _timed_conv_call('wgrad', kmap, cin, cout, x.dtype, 'esb_spconv_wgrad', ptr(x), ptr(dy), ptr(pin),
+                _timed_conv_call('wgrad', kmap, cin, cout, x.dtype, 'esb_spconv_wgrad' + slot, ptr(x), ptr(dy), ptr(pin),
                                  ptr(pout), ptr(koff), ptr(dw), tot, cin, cout, kmap.K, code, stream())
-            if direct:
-                _fire_grad_hooks(weight)
-                dw = None
-            else:
-                dw = dw.view(ctx.wshape)
+            if getattr(weight, '_esb_grad_direct', False):
+                _release_use(weight, direct)
+            dw = None if direct else dw.view(ctx.wshape)
         return dx, dw, None, None, None
 
 
@@ -511,9 +523,9 @@ class _SegNorm(torch.autograd.Function):
         N, C = x.shape
         dy = dy.contiguous()
         gamma, beta = ctx.params
-        direct = (S == 1 and gamma is not None and beta is not None and getattr(gamma, '_esb_grad_direct', False)
-                  and getattr(beta, '_esb_grad_direct', False) and gamma.grad is not None and beta.grad is not None)
-        if direct:   # the column sums ARE d(beta), d(gamma): accumulate them in the arena's (zeroed) gradient slots
+        counted = S == 1 and gamma is not None and beta is not None and ctx.needs_input_grad[2]
+        direct = S == 1 and gamma is not None and beta is not None and _direct(gamma) and _direct(beta)
+        if direct:   # the column sums ARE d(beta), d(gamma): the kernel adds them to the arena's gradient slots
             sg, sgx = beta.grad, gamma.grad
         else:
             sg = torch.empty((S, C), dtype=torch.float32, device=x.device)
@@ -522,8 +534,11 @@ class _SegNorm(torch.autograd.Function):
         dres = torch.empty_like(x) if has_res else None
         call('esb_norm_bwd', ptr(x), ptr(y), ptr(dy), ptr(seg_off), ptr(row_seg), S, N, max_rows, C, ptr(mean), ptr(rstd),
              ptr(g), act, ptr(sg), ptr(sgx), ptr(dx), ptr(dres), 0 if direct else 1, _ffi.dtype_code(x.dtype), stream())
+        if counted:
+            for p in (gamma, beta):
+                if getattr(p, '_esb_grad_direct', False):
+                    _release_use(p, direct)
         if direct:
-            _fire_grad_hooks(gamma, beta)
             return dx, dres, None, None, None, None, None, None, None, None, None, None, None
         if S == 1:       # BatchNorm: the (1,C) sums ARE the parameter gradients (no reduction kernel)
             dgamma = sgx.view(gshape) if gshape is not None else None

@@ -67,6 +67,10 @@ int esb_spconv_fwd(const void* x, const void* w, const int* nbr, void* y, long l
                    int w_transposed, int dtype, void* stream);
 int esb_spconv_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out, const int* k_offsets,
                      float* dw, long long n_pairs_hint, int cin, int cout, int K, int dtype, void* stream);
+/* *_wgrad: dw += the gradient, the add chain starting from dw. *_wgrad_slot: dw = dw + the finished gradient, one rounded add
+ * per element (gradient slots accumulating backward passes, as autograd's `grad += fresh`); equal on a zeroed dw. */
+int esb_spconv_wgrad_slot(const void* x, const void* dy, const int* pair_in, const int* pair_out, const int* k_offsets,
+                          float* dw, long long n_pairs_hint, int cin, int cout, int K, int dtype, void* stream);
 
 /* bf16 tensor-core (wgmma) path of the same operator; masks from esb_kmap_tile_masks;
  * w_layout 0: w (K,cout,cin), 1: w (K,cin,cout) — forward and dgrad read the SAME stored bf16 kernel, no transpose */
@@ -75,6 +79,8 @@ int esb_spconv_tc_fwd(const void* x, const void* wt, const int* nbr, const unsig
                       int cin, int cout, int K, int w_layout, void* stream);
 int esb_spconv_tc_wgrad(const void* x, const void* dy, const int* pair_in, const int* pair_out, const int* k_offsets,
                         float* dw, long long n_pairs_hint, int cin, int cout, int K, void* stream);
+int esb_spconv_tc_wgrad_slot(const void* x, const void* dy, const int* pair_in, const int* pair_out, const int* k_offsets,
+                             float* dw, long long n_pairs_hint, int cin, int cout, int K, void* stream);
 
 /* ---- pooling / normalisation / activation (ME.MinkowskiMaxPooling, InstanceNorm, BatchNorm, ReLU, ELU;
  * mink_resnet.py:64-69, fcaf3d_head.py:923,942,947) -------------------------------------------------------------- */
@@ -92,6 +98,8 @@ int esb_batchnorm_fwd_fused(const void* x, const void* res, long long N, int C, 
                             void* stream);
 int esb_norm_apply(const void* x, const void* res, const int* row_seg, long long N, int C, const float* mean,
                    const float* rstd, const float* gamma, const float* beta, int act, void* y, int dtype, void* stream);
+/* zero_sums 1: sg / sgx (S,C) receive this pass's column sums. zero_sums 0 (S == 1): sg / sgx are gradient slots
+ * (d beta, d gamma) that may hold earlier passes; dx uses this pass's sums only, and each slot becomes slot + sum. */
 int esb_norm_bwd(const void* x, const void* y, const void* dy, const int* seg_off, const int* row_seg, int S,
                  long long N, int max_seg_rows, int C, const float* mean, const float* rstd, const float* gamma, int act,
                  float* sg, float* sgx, void* dx, void* dres, int zero_sums, int dtype, void* stream);
