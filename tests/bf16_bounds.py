@@ -44,6 +44,23 @@ c = 4.2e6), 0.152 for interp_features_kernel, and 0.0015 for the BatchNorm / Ins
 backward carrying the same `fixed` term through the normalisation's backward, `seg_norm_bwd_fixed`). The faults are
 `focal_faults_fwd`, `focal_faults_bwd`, `bias_act_faults`, `act_bwd_faults` and `interp_faults`.
 
+The fp32 instances (the parity arithmetic; the fp32 cases of the three modules) use the same form with out_rel =
+OUT_REL_F32 = 2^-24 and the same C_ACC. Where an fp32 kernel calls rsqrtf or expm1f (the normalisations, ELU), the
+function's documented maximum error (ULP_RSQRTF, ULP_EXPM1F) is an explicit `fixed` term (`seg_norm_fn_fixed`), and the
+ELU backward keeps its `fixed` term for reading the derivative as y + 1, with the fp32 output rounding. On an H100 SXM
+(80 GB HBM3, 132 SMs, 700 W power limit) the worst fp32 ratios were: 0.067 for the SIMT sparse forward / dgrad
+(spconv_fwd_kernel<float, *>, from the stem's dgrad; 0.058 at cin 33 / cout 70, 0.0045 at 640 -> 640), 0.312 for the
+SIMT wgrad (640 -> 640, one split, into a non-zero dw; 0.228 with six splits), 0.0122 for the two-pass normalisations
+(InstanceNorm, C = 64; the BatchNorms below 0.0015), 0.051 for the direct 2-D forward (a 1x1 stride-2 downsample), 0.026
+for its dgrad, 0.0018 for its wgrad (n_red = pixels + slices: its atomics add the pixel slices in any order), and 0.55
+for painting (under C_PAINT). Pooling and the image normalisation are bit-exact in fp32 too, and every fp32 convolution family is bit-exact on
+operands in {-1, 0, 1}. One case needs more than C_ACC: the fp32 forward of the sparse stem (3 input channels), 0.504.
+Its rows sum a few 3-term dot products, too few terms for the roundings of the partial sums to average out. An fma chain
+over n terms is off by at most (n - 1) 2^-24 A beyond the output rounding, a ratio of (n - 1) / n: below 1, the textbook
+constant, which that case uses (C_SHORT_F32). In bf16 the output rounding hides this (0.0034). The new faults are
+`direct_wgrad_slice_faults` (a dropped pixel slice, on integer operands) and `wgrad_faults` at the SIMT split length;
+`simt_wgrad_splits` and `direct_wgrad_slices` mirror the two selection rules.
+
 Nothing here imports the library: it runs on CPU tensors as well as CUDA tensors.
 """
 import math
@@ -55,6 +72,7 @@ OUT_REL_BF16 = 2.0 ** -8
 OUT_REL_F32 = 2.0 ** -24
 C_ACC = 0.5
 C_PAINT = 1.0
+C_SHORT_F32 = 1.0
 
 
 # ------------------------------------------------------------------------------------------------ the bound
@@ -178,11 +196,43 @@ def seg_norm_bwd_ref(x, gy, gamma, st):
     return (dx, A_dx), (dg, A_dg), (db, A_db)
 
 
+# The documented maximum errors of the CUDA single-precision functions the fp32 kernels call (CUDA C++ Programming Guide,
+# "Mathematical Functions", single precision), in ulps; one ulp of an fp32 value v is at most ULP |v|. They enter the fp32
+# bounds as explicit `fixed` terms, not through c.
+ULP = 2.0 ** -23
+ULP_RSQRTF = 2
+ULP_EXPM1F = 1
+
+
+def seg_norm_fn_fixed(x, gamma, st, z, act, gy=None):
+    """What rsqrtf and expm1f may add to an fp32 normalisation beyond the roundings c covers. rstd = rsqrtf(var + eps) is
+    off by e = ULP_RSQRTF ULP relative, which moves z by e |xhat gamma|; ELU's expm1f adds ULP_EXPM1F ULP |y| where z <= 0.
+    With `gy` (dy act'(y)) also the backward: dx = gamma rs (g - mean g - xhat mean(g xhat)) reads rs once and xhat twice
+    (directly and through sum g xhat), so it moves by 3 e |gamma| rs (|g| + mean|g| + |xhat| mean|g xhat|); dgamma =
+    sum g xhat by e sum |g xhat|; dbeta not at all. Returns F_y, or (F_y, F_dx, F_dgamma, F_dbeta)."""
+    seg, n, rs = st['seg'], st['n'], st['rs']
+    e = ULP_RSQRTF * ULP
+    xh = ((x.double() - st['mean'][seg]) * rs[seg]).abs()
+    gm = gamma.double().abs().view(1, -1)
+    F_y = e * xh * gm
+    if act == 2:
+        F_y = F_y + ULP_EXPM1F * ULP * torch.expm1(z.clamp(max=0)).abs()
+    if gy is None:
+        return F_y
+    g = gy.double().abs()
+    S, C = n.shape[0], x.shape[1]
+    P = torch.zeros((S, C), dtype=torch.float64, device=x.device)
+    pa, qa = P.clone().index_add_(0, seg, g) / n, P.clone().index_add_(0, seg, g * xh) / n
+    F_dx = 3 * e * gm * rs[seg] * (g + pa[seg] + xh * qa[seg])
+    return F_y, F_dx, e * (g * xh).sum(0), torch.zeros(C, dtype=torch.float64, device=x.device)
+
+
 # ------------------------------------------------------------------------------------------------ faults
-def conv_faults(out, x, w, nbr, w_layout=1, tile_rows=128):
+def conv_faults(out, x, w, nbr, w_layout=1, tile_rows=128, chunk=64):
     """Copies of a correct gather-GEMM output with one fault each, as a tile kernel could make them:
-    the contribution of the sparsest used kernel offset missing, output channels 0 and 1 swapped, the last 64-channel
-    slice of the reduction missing, and the last (partial) 128-row tile left at zero."""
+    the contribution of the sparsest used kernel offset missing, output channels 0 and 1 swapped, the last `chunk`-channel
+    slice of the reduction (partial when chunk does not divide cin) missing, and the last (partial) `tile_rows`-row tile
+    left at zero."""
     K, n_out = nbr.shape
     assert n_out % tile_rows, 'the last row tile must be partial'
     cin = x.shape[1]
@@ -191,8 +241,9 @@ def conv_faults(out, x, w, nbr, w_layout=1, tile_rows=128):
     one = torch.full_like(nbr, -1)
     one[k_min] = nbr[k_min]
     drop_k = gather_gemm(x, w, one, w_layout)[0]
+    c0 = (cin - 1) // chunk * chunk
     xs = x.clone()
-    xs[:, :cin - 64] = 0
+    xs[:, :c0] = 0
     drop_slice = gather_gemm(xs, w, nbr, w_layout)[0]
     swapped = out.clone()
     swapped[:, [0, 1]] = out[:, [1, 0]]
@@ -200,7 +251,7 @@ def conv_faults(out, x, w, nbr, w_layout=1, tile_rows=128):
     tail[n_out // tile_rows * tile_rows:] = 0
     return [(f'kernel offset {k_min} dropped', (out.double() - drop_k).to(out.dtype)),
             ('output channels 0 and 1 swapped', swapped),
-            (f'reduction channels {cin - 64}..{cin - 1} zeroed', (out.double() - drop_slice).to(out.dtype)),
+            (f'reduction channels {c0}..{cin - 1} zeroed', (out.double() - drop_slice).to(out.dtype)),
             ('last partial row tile left at zero', tail)]
 
 
@@ -238,9 +289,34 @@ def tc_wgrad_chunk_pairs(n_pairs_hint, cin, cout, sms):
     return min(max(cp, 512), 16384)
 
 
-def random_kernel_map(n_in, n_out, K, gen, device='cpu', empty_offset=None, single_offset=None, empty_tile=None):
+def simt_wgrad_splits(n_pairs_hint, K, cin, cout, sms):
+    """The pair splits esb_spconv_wgrad picks (csrc/spconv.cu, spconv_wgrad): ~4 CTAs per SM over the 64 x 64 (cin, cout)
+    tiles of every offset, at least 256 pairs per split on average, 1..64. Split s of an offset with n pairs holds pairs
+    [s per, (s + 1) per) with per = ceil(n / splits) (`simt_wgrad_split_len`); the partials are added in split order."""
+    tiles = K * _cdiv(cin, 64) * _cdiv(cout, 64)
+    splits = min(4 * sms // tiles, (n_pairs_hint // K + 1) // 256 + 1)
+    return min(max(splits, 1), 64)
+
+
+def simt_wgrad_split_len(n_pairs, splits):
+    return _cdiv(n_pairs, splits)
+
+
+def direct_wgrad_slices(M, cin, cout, taps, sms):
+    """(slice, n_slices) esb_conv2d_direct_wgrad picks (csrc/conv2d_direct.cu): enough (256-pair block, tap, slice) CTAs
+    to give each SM ~32, at most 1024 slices, at least 64 output pixels each; slice z holds pixels [z slice, (z+1) slice)
+    of the M = N Ho Wo output pixels and adds its partial to dw with fp32 atomics."""
+    pair_blocks = _cdiv(cin * cout, 256)
+    slices = min(4 * sms * 8 // (pair_blocks * taps) + 1, 1024)
+    slice_len = max(_cdiv(M, slices), 64)
+    return slice_len, _cdiv(M, slice_len)
+
+
+def random_kernel_map(n_in, n_out, K, gen, device='cpu', empty_offset=None, single_offset=None, empty_tile=None,
+                      tile_rows=128):
     """nbr (K, n_out) int32: through each offset an injective map into [0, n_in) of random density (as a real kernel map
-    is); `empty_offset` gets no neighbour at all, `single_offset` exactly one, and the 128 rows of `empty_tile` none."""
+    is); `empty_offset` gets no neighbour at all, `single_offset` exactly one, and the `tile_rows` rows of `empty_tile`
+    none."""
     nbr = torch.full((K, n_out), -1, dtype=torch.int32)
     for k in range(K):
         dens = 0.1 + 0.5 * float(torch.rand((), generator=gen))
@@ -255,7 +331,7 @@ def random_kernel_map(n_in, n_out, K, gen, device='cpu', empty_offset=None, sing
         nbr[single_offset] = -1
         nbr[single_offset, o] = v
     if empty_tile is not None:
-        nbr[:, empty_tile * 128:(empty_tile + 1) * 128] = -1
+        nbr[:, empty_tile * tile_rows:(empty_tile + 1) * tile_rows] = -1
     return nbr.to(device)
 
 
@@ -541,6 +617,17 @@ def wgrad_split_faults(out, x, dy, w_shape, stride, pad, geom):
     dym = dy * (keep if dy.dim() == 5 else keep[:, 0]).unsqueeze(1)
     part = wgrad(x.double(), w_shape, dym.double(), stride, pad)
     return [(f'pixel split {int(split.max())} ({geom["last_split"]} tiles) dropped', (out.double() - part).to(out.dtype))]
+
+
+def direct_wgrad_slice_faults(out, x, dy, w_shape, stride, pad, slice_len):
+    """A correct direct-kernel weight gradient without its last pixel slice (output pixels m >= (slices - 1) slice_len in
+    the (image, row, column) order of conv2d_direct_wgrad_kernel; bf16_bounds.direct_wgrad_slices)."""
+    wgrad = _conv_ops(2)[2]
+    N, _, Ho, Wo = dy.shape
+    m = torch.arange(N * Ho * Wo, device=dy.device).view(N, 1, Ho, Wo)
+    first = (N * Ho * Wo - 1) // slice_len * slice_len
+    part = wgrad(x.double(), w_shape, (dy.double() * (m >= first)), stride, pad)
+    return [(f'pixel slice at {first} dropped', (out.double() - part).to(out.dtype))]
 
 
 def attn_fwd_faults(o, q, k, v, key_pad, scale):

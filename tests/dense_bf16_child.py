@@ -4,26 +4,18 @@ A case whose own checks fail still reports what it launched (the parent run repo
 import json
 import os
 import sys
-import traceback
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 import test_dense_bf16_gpu as T  # noqa: E402
-from sparse_bf16_child import _calls  # noqa: E402
+from sparse_bf16_child import run_cases  # noqa: E402
 
 
 def main():
-    T._CHILD = {}
     census = 'test_step_launches_only_pinned_dense_instances'
     tests = [n for n in dir(T) if n.startswith('test_') and n != census]
-    for name in tests + [census]:
-        for kw in _calls(getattr(T, name)):
-            try:
-                getattr(T, name)(**kw)
-            except Exception:
-                traceback.print_exc(file=sys.stderr)
-    print(json.dumps(T._CHILD))
+    print(json.dumps(run_cases(T, tests + [census])))
 
 
 if __name__ == '__main__':

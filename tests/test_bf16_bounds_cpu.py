@@ -270,3 +270,78 @@ def test_bound_accepts_emulated_interpolation_and_rejects_its_faults():
     B.assert_within(out, ref, A, n_red, B.OUT_REL_F32, 'emulated interpolation')
     assert bool((rows < 0).any() & (rows >= 0).any()) and bool((np.asarray(q)[:, 1:] < 0).any())
     B.assert_rejects(B.interp_faults(out, c, feats, ts, q), ref, A, n_red, B.OUT_REL_F32)
+
+
+# ------------------------------------------------------------------------------------------------ fp32 (parity) kernels
+def test_bound_accepts_emulated_fp32_simt_conv_and_rejects_its_faults():
+    """The fp32 SIMT convolution (64-row tiles, 16-channel reduction chunks) emulated in fp32 passes the bound with the
+    fp32 output rounding, and its faults, the dropped last (partial) 16-channel chunk included, are rejected at C_ACC."""
+    gen = torch.Generator().manual_seed(9)
+    n_in, n_out, K, cin, cout = 400, 300, 27, 40, 70
+    nbr = B.random_kernel_map(n_in, n_out, K, gen, empty_offset=5, single_offset=7, empty_tile=1, tile_rows=64)
+    for w_layout in (1, 0):
+        x = torch.randn(n_in, cin, generator=gen)
+        w = torch.randn((K, cin, cout) if w_layout else (K, cout, cin), generator=gen) / (K * cin) ** 0.5
+        ref, A, n_red = B.gather_gemm(x, w, nbr, w_layout)
+        out = B.gather_gemm(x, w, nbr, w_layout, dtype=torch.float32)[0]
+        B.assert_within(out, ref, A, n_red, B.OUT_REL_F32, f'emulated fp32 conv, layout {w_layout}')
+        assert bool((out[64:128] == 0).all())
+        faults = B.conv_faults(out, x, w, nbr, w_layout, tile_rows=64, chunk=16)
+        assert 'reduction channels 32..39' in faults[2][0]
+        B.assert_rejects(faults, ref, A, n_red, B.OUT_REL_F32)
+
+
+def test_bound_rejects_a_dropped_simt_wgrad_split_in_fp32():
+    """An fp32-emulated SIMT weight gradient (n_red = pairs + splits) passes the bound; with one pair split of an offset
+    missing it is rejected at C_ACC."""
+    gen = torch.Generator().manual_seed(10)
+    K, n_rows, cin, cout = 27, 3000, 64, 64
+    counts = [0, 5] + [int(c) for c in torch.randint(1, n_rows + 1, (K - 2, ), generator=gen)]
+    splits = B.simt_wgrad_splits(sum(counts), K, cin, cout, 132)
+    assert splits == 6 and B.simt_wgrad_splits(sum(counts), K, 640, 640, 132) == 1
+    pin, pout, koff = B.random_pairs(counts, n_rows, n_rows, gen)
+    x, dy = torch.randn(n_rows, cin, generator=gen), torch.randn(n_rows, cout, generator=gen)
+    ref, A, n_red = B.pair_wgrad(x, dy, pin, pout, koff)
+    out = B.pair_wgrad(x, dy, pin, pout, koff, dtype=torch.float32)[0]
+    B.assert_within(out, ref, A, n_red + splits, B.OUT_REL_F32, 'emulated fp32 wgrad')
+    faults = B.wgrad_faults(out, x, dy, pin, pout, koff, B.simt_wgrad_split_len(max(counts), splits))
+    B.assert_rejects(faults, ref, A, n_red + splits, B.OUT_REL_F32)
+
+
+def test_bound_rejects_a_dropped_direct_wgrad_pixel_slice():
+    """The direct fp32 weight gradient on operands in {-1, 0, 1} is exact whatever order its atomics add the pixel slices
+    in; the same without its last pixel slice is rejected at C_ACC (n_red = pixels + slices)."""
+    gen = torch.Generator().manual_seed(11)
+    n, cin, cout, hw = 2, 24, 40, (31, 45)
+    M = n * hw[0] * hw[1]
+    slice_len, n_slices = B.direct_wgrad_slices(M, cin, cout, 9, 132)
+    assert (slice_len, n_slices) == (64, 44)
+    assert B.direct_wgrad_slices(M, 3, 16, 49, 132) == (64, 44) and B.direct_wgrad_slices(10 ** 6, 64, 64, 9, 132)[1] == 30
+    d = (16.0 / M) ** 0.5
+    x, dy = B.ternary((n, cin) + hw, d, gen), B.ternary((n, cout) + hw, d, gen)
+    ref, A, n_red = B.dense_wgrad_ref(x, dy, (cout, cin, 3, 3), 1, 1)
+    out = torch.nn.grad.conv2d_weight(x, (cout, cin, 3, 3), dy, 1, 1)
+    B.assert_exact(out, ref, A, 'emulated direct wgrad', out_bf16=False)
+    faults = B.direct_wgrad_slice_faults(out, x, dy, (cout, cin, 3, 3), 1, 1, slice_len)
+    assert f'at {(n_slices - 1) * slice_len}' in faults[0][0]
+    B.assert_rejects(faults, ref, A, n_red + n_slices, B.OUT_REL_F32)
+
+
+def test_fp32_norm_bound_accepts_emulated_norm():
+    """An fp32 InstanceNorm + ELU emulated in fp32 (torch's rsqrt and expm1) passes the bound with the documented function
+    errors as fixed terms (bf16_bounds.seg_norm_fn_fixed); channel 0 with the wrong rstd is rejected."""
+    gen = torch.Generator().manual_seed(12)
+    sizes, C = [300, 37, 129], 12
+    x = torch.randn(sum(sizes), C, generator=gen) * 2 + 0.5
+    gamma, beta = torch.rand(C, generator=gen) + 0.5, torch.randn(C, generator=gen)
+    z, A, n_red, st = B.seg_norm_ref(x, sizes, gamma, beta, 1e-8)
+    seg = st['seg']
+    mean = torch.zeros(len(sizes), C).index_add_(0, seg, x) / torch.tensor(sizes, dtype=torch.float32).view(-1, 1)
+    d = x - mean[seg]
+    var = torch.zeros(len(sizes), C).index_add_(0, seg, d * d) / torch.tensor(sizes, dtype=torch.float32).view(-1, 1)
+    y = B._act(d * torch.rsqrt(var + 1e-8)[seg] * gamma + beta, 2)
+    F_y = B.seg_norm_fn_fixed(x, gamma, st, z, 2)
+    B.assert_within(y, B._act(z, 2), A, n_red, B.OUT_REL_F32, 'emulated fp32 norm', fixed=F_y)
+    bad = y.clone()
+    bad[:, 0] = B._act(d[:, 0] * torch.rsqrt(var[:, 0] + 1e-4)[seg] * gamma[0] + beta[0], 2)
+    B.assert_rejects([('rstd of channel 0 off', bad)], B._act(z, 2), A, n_red, B.OUT_REL_F32, F_y)

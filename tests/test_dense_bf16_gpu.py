@@ -1,7 +1,8 @@
-"""Every bf16 kernel instance of the dense branch of the training steps (the per-view image backbone, point painting, the
-occupancy Conv3d neck, the grounding attention), pinned per element against a float64 reference on the same bf16 operands
-(tests/bf16_bounds.py), at sizes derived from the device's SM count so each case reaches the geometry it names. Outputs are
-pre-filled with NaN: an element no CTA writes fails. Each conv case also runs on operands in {-1, 0, 1}, where the result
+"""Every bf16 and fp32 kernel instance of the dense branch of the training steps (the per-view image backbone, point
+painting, the occupancy Conv3d neck, the grounding attention), pinned per element against a float64 reference on the same
+operands (tests/bf16_bounds.py), at sizes derived from the device's SM count so each case reaches the geometry it names.
+fp32 is the parity arithmetic: every fp32 2-D convolution runs on the SIMT direct kernels (conv2d_direct.cu), all three
+passes, and painting runs its fp32 instances. Outputs are pre-filled with NaN: an element no CTA writes fails. Each conv case also runs on operands in {-1, 0, 1}, where the result
 must equal the reference bit for bit however long the reduction; the split sums (conv wgrad, attention dQ) are checked
 to be added in split order, bit for bit. Each case runs under torch.profiler (in a fresh interpreter, see
 dense_bf16_child.py) and asserts that the instance it claims was launched; the census tests assert that the C2, C3 and
@@ -22,7 +23,16 @@ import bf16_bounds as B
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
 BF = torch.bfloat16
+F32 = torch.float32
 NAN = float('nan')
+
+
+def _t(dtype):
+    return '__nv_bfloat16' if dtype == BF else 'float'
+
+
+def _out_rel(dtype):
+    return B.OUT_REL_BF16 if dtype == BF else B.OUT_REL_F32
 
 
 def _sms():
@@ -86,6 +96,11 @@ ATTN = ['attn_fwd_kernel', 'attn_delta_kernel', 'attn_bwd_kernel']
 PAINT = ['paint_fwd_kernel<__nv_bfloat16>', 'paint_bwd_pairs_kernel<__nv_bfloat16>', 'paint_bwd_sum_kernel<__nv_bfloat16>']
 PINNED = {CONV(n, mn) for n in (16, 32, 64, 128) for mn in (False, True)} | {WGRAD(n) for n in (16, 32, 64, 128)} | \
     {STEM, DIRECT_FWD, DIRECT_DGRAD} | set(POOL.values()) | set(ATTN) | set(PAINT)
+DIRECT_FWD_F32, DIRECT_DGRAD_F32 = 'conv2d_direct_fwd_kernel<float>', 'conv2d_direct_dgrad_kernel<float>'
+DIRECT_WGRAD_F32 = 'conv2d_direct_wgrad_kernel<float>'
+POOL_F32 = 'maxpool2d_nhwc_kernel<float, 1>'
+PAINT_F32 = [s.replace('__nv_bfloat16', 'float') for s in PAINT]
+PINNED_F32 = {DIRECT_FWD_F32, DIRECT_DGRAD_F32, DIRECT_WGRAD_F32, POOL_F32} | set(PAINT_F32)
 
 
 # ------------------------------------------------------------------------------------------------ calls
@@ -335,13 +350,13 @@ def test_conv_tma_wgrad_split_order(name):
 
 
 # ------------------------------------------------------------------------------------------------ non-tensor-map bodies
-def _small_operands(xs, ws, exact, gen, n_red):
+def _small_operands(xs, ws, exact, gen, n_red, dtype=BF):
     """Random operands, or operands in {-1, 0, 1} (integer bias) with partial sums around 16."""
     if exact:
         d = min(0.5, (16.0 / n_red) ** 0.5)
-        return (B.ternary(xs, d, gen).to(DEV, BF), B.ternary(ws, d, gen).to(DEV, BF),
+        return (B.ternary(xs, d, gen).to(DEV, dtype), B.ternary(ws, d, gen).to(DEV, dtype),
                 torch.randint(-4, 5, (ws[0], ), generator=gen).float().to(DEV))
-    return (torch.randn(xs, generator=gen).to(DEV, BF), (torch.randn(ws, generator=gen) / n_red ** 0.5).to(DEV, BF),
+    return (torch.randn(xs, generator=gen).to(DEV, dtype), (torch.randn(ws, generator=gen) / n_red ** 0.5).to(DEV, dtype),
             torch.randn(ws[0], generator=gen).to(DEV))
 
 
@@ -369,52 +384,199 @@ def test_stem7x7(n, hw, exact):
     print(f'ratio {r:.4g}')
 
 
-@pytest.mark.parametrize('exact', [False, True], ids=['random', 'exact'])
-def test_direct_fwd_c3_stem(exact):
-    """conv2d_direct_fwd_kernel<bf16>: C3's 3 -> 64 7x7 / 2 stem (base_channels 64 is neither the stem kernel's width nor
-    TMA-sized, so backbones._ConvBlock2D sends it here), with bias and ReLU, into a NaN-filled output."""
+def _direct_fwd(x, w, b, res, stride, pad, relu):
+    """esb_conv2d_direct_fwd: x (N, Cin, H, W), w (Cout, Cin, k, k) -> (N, Cout, Ho, Wo) written into NaN."""
     from embodiedscan_b200._ffi import call, dtype_code, ptr, stream
+    n, cin, H, W = x.shape
+    cout, k = w.shape[0], w.shape[2]
+    y = _nan((n, *_out_size((H, W), k, stride, pad), cout), x.dtype)
+    xc, wc, rc = _cl(x), _cl(w), _cl(res) if res is not None else None     # held until the launch
+    call('esb_conv2d_direct_fwd', ptr(xc), ptr(wc), ptr(b), ptr(rc), ptr(y), n, H, W, cin, cout, k, k, stride, pad,
+         int(relu), dtype_code(x.dtype), stream())
+    return y.movedim(-1, 1)
+
+
+def _direct_dgrad(dy, w, x_shape, stride, pad):
+    from embodiedscan_b200._ffi import call, dtype_code, ptr, stream
+    n, cin, H, W = x_shape
+    cout, k = w.shape[0], w.shape[2]
+    dx = _nan((n, H, W, cin), dy.dtype)
+    dyc, wc = _cl(dy), _cl(w)
+    call('esb_conv2d_direct_dgrad', ptr(dyc), ptr(wc), ptr(dx), n, H, W, cin, cout, k, k, stride, pad,
+         dtype_code(dy.dtype), stream())
+    return dx.movedim(-1, 1)
+
+
+def _direct_wgrad(x, dy, w_shape, stride, pad):
+    """esb_conv2d_direct_wgrad into zeros (its pixel slices add with atomics onto a zeroed dw): (Cout, Cin, k, k) fp32."""
+    from embodiedscan_b200._ffi import call, dtype_code, ptr, stream
+    n, cin, H, W = x.shape
+    cout, k = w_shape[0], w_shape[2]
+    dw = torch.zeros((cout, k, k, cin), device=DEV)
+    xc, dyc = _cl(x), _cl(dy)
+    call('esb_conv2d_direct_wgrad', ptr(xc), ptr(dyc), ptr(dw), n, H, W, cin, cout, k, k, stride, pad, dtype_code(x.dtype),
+         stream())
+    return dw.permute(0, 3, 1, 2)
+
+
+@pytest.mark.parametrize('exact', [False, True], ids=['random', 'exact'])
+@pytest.mark.parametrize('dtype', [BF, F32], ids=['bf16', 'fp32'])
+def test_direct_fwd_c3_stem(dtype, exact):
+    """conv2d_direct_fwd_kernel<bf16> and <float>: C3's 3 -> 64 7x7 / 2 stem (base_channels 64 is neither the stem kernel's
+    width nor TMA-sized, so backbones._ConvBlock2D sends it here; in fp32 every convolution comes here), with bias and
+    ReLU, into a NaN-filled output."""
     gen = torch.Generator().manual_seed(64 + exact)
     n, hw = 2, (62, 90)
-    x, w, b = _small_operands((n, 3, *hw), (64, 3, 7, 7), exact, gen, 147)
-    y = _nan((n, *_out_size(hw, 7, 2, 3), 64))
-    xc, wc = _cl(x), _cl(w)
-    _, seen = _instances(lambda: call('esb_conv2d_direct_fwd', ptr(xc), ptr(wc), ptr(b), None, ptr(y), n, *hw, 3, 64, 7,
-                                      7, 2, 3, 1, dtype_code(BF), stream()))
-    _claim(seen, [DIRECT_FWD], f'direct fwd C3 stem {exact}')
+    x, w, b = _small_operands((n, 3, *hw), (64, 3, 7, 7), exact, gen, 147, dtype)
+    y, seen = _instances(lambda: _direct_fwd(x, w, b, None, 2, 3, True))
+    _claim(seen, [DIRECT_FWD if dtype == BF else DIRECT_FWD_F32], f'direct fwd C3 stem {exact}' + ('' if dtype == BF else ' fp32'))
     pre, A, n_red = B.dense_conv_ref(x, w, 2, 3, b)
-    y = y.movedim(-1, 1)
     if exact:
-        B.assert_exact(y, pre.clamp(min=0), A, 'direct fwd')
+        B.assert_exact(y, pre.clamp(min=0), A, 'direct fwd', out_bf16=dtype == BF)
         return
-    r = B.assert_within(y, pre.clamp(min=0), A, n_red, B.OUT_REL_BF16, 'direct fwd')
-    B.assert_rejects(B.conv_fwd_faults(y, pre, x, w, 2, 3, True, (1, 1, 1, 1)), pre.clamp(min=0), A, n_red,
-                     B.OUT_REL_BF16)
+    r = B.assert_within(y, pre.clamp(min=0), A, n_red, _out_rel(dtype), 'direct fwd')
+    B.assert_rejects(B.conv_fwd_faults(y, pre, x, w, 2, 3, True, (1, 1, 1, 1)), pre.clamp(min=0), A, n_red, _out_rel(dtype))
     print(f'ratio {r:.4g}')
 
 
 @pytest.mark.parametrize('exact', [False, True], ids=['random', 'exact'])
-def test_direct_dgrad_stride3(exact):
-    """conv2d_direct_dgrad_kernel<bf16>: the input gradient of a stride-3 convolution with TMA-sized channels (the TMA
-    dgrad takes strides 1 and 2 only), into a NaN-filled output."""
-    from embodiedscan_b200._ffi import call, dtype_code, ptr, stream
+@pytest.mark.parametrize('dtype', [BF, F32], ids=['bf16', 'fp32'])
+def test_direct_dgrad_stride3(dtype, exact):
+    """conv2d_direct_dgrad_kernel<bf16> and <float>: the input gradient of a stride-3 convolution with TMA-sized channels
+    (the TMA dgrad takes strides 1 and 2 only; in fp32 every dgrad comes here), into a NaN-filled output."""
     cin, cout, k, stride, pad, hw, n = 64, 64, 3, 3, 1, (31, 41), 2
     gen = torch.Generator().manual_seed(3 + exact)
-    dy, w, _ = _small_operands((n, cout, *_out_size(hw, k, stride, pad)), (cout, cin, k, k), exact, gen, k * k * cout)
-    dx = _nan((n, *hw, cin))
-    dyc, wc = _cl(dy), _cl(w)
-    _, seen = _instances(lambda: call('esb_conv2d_direct_dgrad', ptr(dyc), ptr(wc), ptr(dx), n, *hw, cin, cout, k, k,
-                                      stride, pad, dtype_code(BF), stream()))
-    _claim(seen, [DIRECT_DGRAD], f'direct dgrad stride 3 {exact}')
+    dy, w, _ = _small_operands((n, cout, *_out_size(hw, k, stride, pad)), (cout, cin, k, k), exact, gen, k * k * cout, dtype)
+    dx, seen = _instances(lambda: _direct_dgrad(dy, w, (n, cin, *hw), stride, pad))
+    _claim(seen, [DIRECT_DGRAD if dtype == BF else DIRECT_DGRAD_F32],
+           f'direct dgrad stride 3 {exact}' + ('' if dtype == BF else ' fp32'))
     ref, A, n_red = B.dense_dgrad_ref(dy, w, (n, cin, *hw), stride, pad)
-    dx = dx.movedim(-1, 1)
     if exact:
-        B.assert_exact(dx, ref, A, 'direct dgrad')
+        B.assert_exact(dx, ref, A, 'direct dgrad', out_bf16=dtype == BF)
         return
-    r = B.assert_within(dx, ref, A, n_red, B.OUT_REL_BF16, 'direct dgrad')
+    r = B.assert_within(dx, ref, A, n_red, _out_rel(dtype), 'direct dgrad')
     B.assert_rejects(B.conv_dgrad_faults(dx, ref, dy, w, (n, cin, *hw), stride, pad, (1, 1, 1, 1)), ref, A, n_red,
-                     B.OUT_REL_BF16)
+                     _out_rel(dtype))
     print(f'ratio {r:.4g}')
+
+
+# fp32 direct convolutions at the backbone's own shapes (ResNet-18 / base 16 of C1: widths 16..128), (cin, cout, k, stride,
+# pad, (H, W), images, residual). Forward: cin 24 puts the 64-element filter chunks across tap boundaries (216 = 3 x 64 + 24)
+# and cout 40 is not a multiple of the 16 output channels of a thread; the 128-pixel blocks end partial.
+DIRECT_FWD_CASES = {
+    '3x3_s1_c24_c40_res': (24, 40, 3, 1, 1, (31, 45), 2, True),
+    '3x3_s2_odd': (16, 32, 3, 2, 1, (33, 47), 2, False),
+    '1x1_s2_ds': (64, 128, 1, 2, 0, (31, 45), 2, False),
+    '3x3_s1_c128_res': (128, 128, 3, 1, 1, (15, 21), 3, True),
+}
+
+
+@pytest.mark.parametrize('exact', [False, True], ids=['random', 'exact'])
+@pytest.mark.parametrize('name', list(DIRECT_FWD_CASES))
+def test_direct_fwd_f32(name, exact):
+    """conv2d_direct_fwd_kernel<float> with bias (+ residual) + ReLU as _ConvBlock2D calls it in fp32, into NaN."""
+    cin, cout, k, stride, pad, hw, n, res = DIRECT_FWD_CASES[name]
+    gen = torch.Generator().manual_seed(sum(map(ord, name)) + exact)
+    x, w, b = _small_operands((n, cin, *hw), (cout, cin, k, k), exact, gen, k * k * cin, F32)
+    ys = (n, cout, *_out_size(hw, k, stride, pad))
+    r = (torch.randint(-4, 5, ys, generator=gen).float() if exact else torch.randn(ys, generator=gen)).to(DEV) \
+        if res else None
+    y, seen = _instances(lambda: _direct_fwd(x, w, b, r, stride, pad, True))
+    _claim(seen, [DIRECT_FWD_F32], f'direct fwd fp32 {name} {exact}')
+    assert (n * ys[2] * ys[3]) % 128, 'the last 128-pixel block must be partial'
+    pre, A, n_red = B.dense_conv_ref(x, w, stride, pad, b, r)
+    if exact:
+        B.assert_exact(y, pre.clamp(min=0), A, f'direct fwd {name}', out_bf16=False)
+        return
+    ratio = B.assert_within(y, pre.clamp(min=0), A, n_red, B.OUT_REL_F32, f'direct fwd {name}')
+    B.assert_rejects(B.conv_fwd_faults(y, pre, x, w, stride, pad, True, (1, 1, 1, 1)), pre.clamp(min=0), A, n_red,
+                     B.OUT_REL_F32)
+    print(f'ratio {ratio:.4g}')
+
+
+# dgrad: the reduction runs over cout in 64-channel chunks; cout 80 and 96 end on a partial chunk. (cin, cout, k, stride,
+# pad, (H, W), images)
+DIRECT_DGRAD_CASES = {
+    '3x3_s1_c80': (32, 80, 3, 1, 1, (31, 45), 2),
+    '3x3_s2_odd_c96': (16, 96, 3, 2, 1, (33, 47), 2),
+    '1x1_s2_ds': (64, 128, 1, 2, 0, (31, 45), 2),
+}
+
+
+@pytest.mark.parametrize('exact', [False, True], ids=['random', 'exact'])
+@pytest.mark.parametrize('name', list(DIRECT_DGRAD_CASES))
+def test_direct_dgrad_f32(name, exact):
+    """conv2d_direct_dgrad_kernel<float> (one thread per input pixel and 16 input channels), into NaN. In the 1x1 stride-2
+    case only the even pixels are reached by a tap: dx at every pixel with an odd row or column must be exactly 0."""
+    cin, cout, k, stride, pad, hw, n = DIRECT_DGRAD_CASES[name]
+    gen = torch.Generator().manual_seed(sum(map(ord, name)) + exact)
+    dy, w, _ = _small_operands((n, cout, *_out_size(hw, k, stride, pad)), (cout, cin, k, k), exact, gen, k * k * cout, F32)
+    dx, seen = _instances(lambda: _direct_dgrad(dy, w, (n, cin, *hw), stride, pad))
+    _claim(seen, [DIRECT_DGRAD_F32], f'direct dgrad fp32 {name} {exact}')
+    if k == 1 and stride == 2:
+        odd = torch.ones(hw, dtype=torch.bool, device=DEV)
+        odd[0::2, 0::2] = False
+        assert bool((dx[:, :, odd] == 0).all()), 'pixels no tap reaches must be exactly 0'
+    ref, A, n_red = B.dense_dgrad_ref(dy, w, (n, cin, *hw), stride, pad)
+    if exact:
+        B.assert_exact(dx, ref, A, f'direct dgrad {name}', out_bf16=False)
+        return
+    r = B.assert_within(dx, ref, A, n_red, B.OUT_REL_F32, f'direct dgrad {name}')
+    B.assert_rejects(B.conv_dgrad_faults(dx, ref, dy, w, (n, cin, *hw), stride, pad, (1, 1, 1, 1)), ref, A, n_red,
+                     B.OUT_REL_F32)
+    print(f'ratio {r:.4g}')
+
+
+# wgrad: (cin, cout, k, stride, pad, (H, W), images as a function of the SM count). cin x cout 960 and 3 x 16 are not
+# multiples of the 256-pair block; the 1 x 3 images leave the taps of the first and last filter rows empty (padding only)
+DIRECT_WGRAD_CASES = {
+    '3x3_s1_c24_c40': (24, 40, 3, 1, 1, (31, 45), lambda sms: 2),
+    '3x3_s2_c32_c64': (32, 64, 3, 2, 1, (33, 47), lambda sms: 2),
+    '1x1_s2_ds': (64, 128, 1, 2, 0, (31, 45), lambda sms: 2),
+    'stem_7x7_s2': (3, 16, 7, 2, 3, (62, 90), lambda sms: 2),
+    'tiny_1x3': (16, 16, 3, 1, 1, (1, 3), lambda sms: sms),
+}
+
+
+@pytest.mark.parametrize('exact', [False, True], ids=['random', 'exact'])
+@pytest.mark.parametrize('name', list(DIRECT_WGRAD_CASES))
+def test_direct_wgrad_f32(name, exact):
+    """conv2d_direct_wgrad_kernel<float>: one thread per (cin, cout) pair of a tap, one CTA column per slice of output
+    pixels (bf16_bounds.direct_wgrad_slices), the slices meeting in fp32 atomicAdd on a zeroed dw. The atomics make the
+    order of the slice sums (and so the last bits) run-dependent: on random operands only the bound holds, with
+    n_red = pixels + slices; on operands in {-1, 0, 1} every partial sum is an exact integer, so the result must equal
+    float64 bit for bit whatever the order, and dropping one pixel slice must fail the bound. Taps that padding leaves
+    without a pixel must be exactly 0."""
+    cin, cout, k, stride, pad, hw, n_of = DIRECT_WGRAD_CASES[name]
+    sms = _sms()
+    n = n_of(sms)
+    So = _out_size(hw, k, stride, pad)
+    M = n * So[0] * So[1]
+    slice_len, n_slices = B.direct_wgrad_slices(M, cin, cout, k * k, sms)
+    assert n_slices > 1, (slice_len, n_slices)
+    gen = torch.Generator().manual_seed(sum(map(ord, name)) + exact)
+    xs, ys = (n, cin, *hw), (n, cout, *So)
+    if exact:
+        d = min(0.5, (16.0 / M) ** 0.5)
+        x, dy = B.ternary(xs, d, gen), B.ternary(ys, d, gen)
+    else:
+        x, dy = torch.randn(xs, generator=gen), torch.randn(ys, generator=gen)
+    x, dy = x.to(DEV), dy.to(DEV)
+    wshape = (cout, cin, k, k)
+    dw, seen = _instances(lambda: _direct_wgrad(x, dy, wshape, stride, pad))
+    _claim(seen, [DIRECT_WGRAD_F32], f'direct wgrad fp32 {name} {exact}')
+    ref, A, n_red = B.dense_wgrad_ref(x, dy, wshape, stride, pad)
+    empty = A.sum((0, 1)) == 0
+    if name == 'tiny_1x3':
+        assert bool(empty[0].all() and empty[2].all()), 'the first and last filter rows must see padding only'
+    assert bool((dw[:, :, empty] == 0).all()), 'a tap without pixels must be exactly 0'
+    if exact:
+        B.assert_exact(dw, ref, A, f'direct wgrad {name}', out_bf16=False)
+        B.assert_rejects(B.direct_wgrad_slice_faults(dw, x, dy, wshape, stride, pad, slice_len), ref, A, n_red + n_slices,
+                         B.OUT_REL_F32)
+        return
+    r = B.assert_within(dw, ref, A, n_red + n_slices, B.OUT_REL_F32, f'direct wgrad {name}')
+    print(f'{n_slices} slices of {slice_len} pixels, ratio {r:.4g}')
 
 
 def test_stride3_block_dispatch():
@@ -447,17 +609,19 @@ def test_stride3_block_dispatch():
 
 
 @pytest.mark.parametrize('C', [64, 16, 12])
-def test_maxpool2d_bit_equal(C):
-    """maxpool2d_nhwc_kernel<bf16, 8> (C a multiple of 8) and <bf16, 1>: the stem's 3x3 / 2 / 1 pooling into a NaN-filled
-    output, bit-equal to F.max_pool2d, on an odd extent and values with many ties."""
+@pytest.mark.parametrize('dtype', [BF, F32], ids=['bf16', 'fp32'])
+def test_maxpool2d_bit_equal(dtype, C):
+    """maxpool2d_nhwc_kernel<bf16, 8> (C a multiple of 8), <bf16, 1> and <float, 1> (every fp32 C): the stem's 3x3 / 2 / 1
+    pooling into a NaN-filled output, bit-equal to F.max_pool2d, on an odd extent and values with many ties."""
     from embodiedscan_b200._ffi import call, dtype_code, ptr, stream
     gen = torch.Generator().manual_seed(C)
-    x = torch.randint(-3, 4, (3, C, 31, 45), generator=gen).to(DEV, BF) * 0.5
-    y = _nan((3, *_out_size((31, 45), 3, 2, 1), C))
+    x = torch.randint(-3, 4, (3, C, 31, 45), generator=gen).to(DEV, dtype) * 0.5
+    y = _nan((3, *_out_size((31, 45), 3, 2, 1), C), dtype)
     xc = _cl(x)
-    _, seen = _instances(lambda: call('esb_maxpool2d_nhwc', ptr(xc), ptr(y), 3, 31, 45, C, 3, 2, 1, dtype_code(BF),
+    _, seen = _instances(lambda: call('esb_maxpool2d_nhwc', ptr(xc), ptr(y), 3, 31, 45, C, 3, 2, 1, dtype_code(dtype),
                                       stream()))
-    _claim(seen, [POOL[8 if C % 8 == 0 else 1]], f'maxpool C {C}')
+    _claim(seen, [POOL[8 if C % 8 == 0 else 1] if dtype == BF else POOL_F32],
+           f'maxpool C {C}' + ('' if dtype == BF else ' fp32'))
     assert torch.equal(y.movedim(-1, 1), F.max_pool2d(x, 3, 2, 1))
 
 
@@ -511,7 +675,7 @@ def test_occupancy_conv3d_module(name):
 
 
 # ------------------------------------------------------------------------------------------------ point painting
-def _paint_case(C, path, gen):
+def _paint_case(C, path, gen, dtype=BF):
     """Two scans of 37 views (more than one warp of views) on a 30 x 40 feature map; every view a translation by an odd
     multiple of 1/8 (so no point lies on a pixel boundary), about a fifth of them behind the camera; points on a
     quarter grid reaching past every border, so the sum and the divisor differ (bf16_bounds.paint_ref)."""
@@ -532,8 +696,8 @@ def _paint_case(C, path, gen):
                         torch.randint(-40, 4 * (Hf + 10), (N, ), generator=gen),
                         torch.randint(0, 8, (N, ), generator=gen)], 1)
     pts = cxyz.double() * 0.25
-    feat = torch.randn(Bn * V, Hf, Wf, C, generator=gen).to(DEV, BF)
-    dout = torch.randn(N, C, generator=gen).to(DEV, BF)
+    feat = torch.randn(Bn * V, Hf, Wf, C, generator=gen).to(DEV, dtype)
+    dout = torch.randn(N, C, generator=gen).to(DEV, dtype)
     coords = torch.cat([batch[:, None], cxyz.to(torch.int32)], 1).contiguous().to(DEV) if path == 'coords' else None
     fpts = pts.float().contiguous().to(DEV) if path == 'fpts' else None
     return dict(Bn=Bn, V=V, Hf=Hf, Wf=Wf, N=N, tx=tx.to(DEV), ty=ty.to(DEV), front=front.to(DEV), proj=proj.to(DEV),
@@ -542,43 +706,49 @@ def _paint_case(C, path, gen):
 
 @pytest.mark.parametrize('path', ['coords', 'fpts'])
 @pytest.mark.parametrize('C', [64, 300])
-def test_paint(C, path):
-    """paint_fwd_kernel<bf16> and paint_bwd_pairs / paint_bwd_sum_kernel<bf16> (nearest-pixel painting of voxel rows
-    (coords) or explicit fp32 points (fpts), C up to 512 in 16 slices per lane) against float64 painting: the forward into
-    a NaN-filled output, its per-point count of valid views exactly, the backward into zeros and added onto a non-zero
-    gradient (esb_paint_bwd documents +=)."""
+@pytest.mark.parametrize('dtype', [BF, F32], ids=['bf16', 'fp32'])
+def test_paint(dtype, C, path):
+    """paint_fwd_kernel and paint_bwd_pairs / paint_bwd_sum_kernel, bf16 and fp32 features (nearest-pixel painting of voxel
+    rows (coords, the detector) or explicit fp32 points (fpts, the occupancy prior), C up to 512 in 16 slices per lane)
+    against float64 painting: the forward into a NaN-filled output, its per-point count of valid views exactly, the
+    backward into zeros and added onto a non-zero gradient (esb_paint_bwd documents +=). Both dtypes keep C_PAINT."""
     from embodiedscan_b200._ffi import call, dtype_code, ptr, stream
     gen = torch.Generator().manual_seed(C + len(path))
-    c = _paint_case(C, path, gen)
+    c = _paint_case(C, path, gen, dtype)
     N, V, Hf, Wf = c['N'], c['V'], c['Hf'], c['Wf']
     pad_h, pad_w = float(Hf - 1), float(Wf - 1)
     fb = c['batch'] if path == 'fpts' else None
-    out = _nan((N, C))
+    out = _nan((N, C), dtype)
     cnt = torch.full((N, ), -1, dtype=torch.int32, device=DEV)
     dfeat = torch.zeros((c['Bn'] * V, Hf, Wf, C), device=DEV)
     dw0 = torch.randn(dfeat.shape, generator=gen).to(DEV)
     acc = dw0.clone()
     args = (ptr(c['coords']), ptr(c['fpts']), ptr(fb), N, 0.25 if path == 'coords' else 1.0, ptr(c['metas']), ptr(c['proj']), V)
 
-    def run():
-        call('esb_paint_fwd', *args, ptr(c['feat']), Hf, Wf, C, pad_h, pad_w, ptr(out), ptr(cnt), dtype_code(BF), stream())
+    def fwd():
+        call('esb_paint_fwd', *args, ptr(c['feat']), Hf, Wf, C, pad_h, pad_w, ptr(out), ptr(cnt), dtype_code(dtype),
+             stream())
+
+    def bwd():
         for d in (dfeat, acc):
-            call('esb_paint_bwd', *args, ptr(c['dout']), Hf, Wf, C, pad_h, pad_w, ptr(d), dtype_code(BF), stream())
-    _, seen = _instances(run)
-    _claim(seen, PAINT, f'paint C {C} {path}')
+            call('esb_paint_bwd', *args, ptr(c['dout']), Hf, Wf, C, pad_h, pad_w, ptr(d), dtype_code(dtype), stream())
+    # two sessions: a session whose only kernel the profiler missed records nothing and is run again (_instances), which
+    # only the forward (it overwrites its output) may be
+    seen = _instances(fwd)[1] | _instances(bwd)[1]
+    _claim(seen, PAINT if dtype == BF else PAINT_F32, f'paint C {C} {path}' + ('' if dtype == BF else ' fp32'))
     ref = B.paint_ref(c['feat'], c['pts'], c['batch'], c['tx'], c['ty'], c['front'], (pad_h, pad_w), c['dout'])
     hit, valid = ref['hit'], ref['valid']
     assert bool((hit & ~valid).any()) and bool((hit.sum(1) == 0).any()) and int(hit.sum(1).max()) > 1
     assert torch.equal(cnt.long(), valid.sum(1)), 'valid-view counts differ'
     val, A, n_red = ref['fwd']
-    r = B.assert_within(out, val, A, n_red, B.OUT_REL_BF16, 'paint fwd', c=B.C_PAINT)
+    r = B.assert_within(out, val, A, n_red, _out_rel(dtype), 'paint fwd', c=B.C_PAINT)
     dval, dA, dn = ref['bwd']
     flat = lambda t: t.reshape(-1, C)  # noqa: E731
     r = max(r, B.assert_within(flat(dfeat), dval, dA, dn, B.OUT_REL_F32, 'paint bwd', c=B.C_PAINT))
     r = max(r, B.assert_within(flat(acc), flat(dw0).double() + dval, flat(dw0).double().abs() + dA, dn + 1, B.OUT_REL_F32,
                                'paint bwd onto a non-zero gradient', c=B.C_PAINT))
     fwd_f, bwd_f = B.paint_faults(out, flat(dfeat), ref, c['feat'], c['dout'])
-    B.assert_rejects(fwd_f, val, A, n_red, B.OUT_REL_BF16, c=B.C_PAINT)
+    B.assert_rejects(fwd_f, val, A, n_red, _out_rel(dtype), c=B.C_PAINT)
     B.assert_rejects(bwd_f, dval, dA, dn, B.OUT_REL_F32, c=B.C_PAINT)
     print(f'ratio {r:.4g}')
 
@@ -707,10 +877,11 @@ def _step(model, batch):
     sum(losses.values()).backward()
 
 
-def census_step(variant):
-    """(model, batch) of the census step of `variant` in bf16 training mode. C3 / C4 keep the published channel widths
-    (which, with the strides, decide every instance: conv_tma_run, conv_wgrad_any, _ConvBlock2D) on one or two scans of
-    two small views. Shared with the whole-library census of test_head_elementwise_bf16_gpu.py."""
+def census_step(variant, dtype=BF):
+    """(model, batch) of the census step of `variant` in training mode with compute dtype `dtype`. C3 / C4 keep the
+    published channel widths (which, with the strides, decide every instance: conv_tma_run, conv_wgrad_any, _ConvBlock2D)
+    on one or two scans of two small views; C1 (the fp32 parity detector) runs on the batch of test_model_gpu.py's fp32
+    training cases. Shared with the whole-library census of test_head_elementwise_bf16_gpu.py."""
     import warnings
     from embodiedscan_b200 import MODELS
     from embodiedscan_b200 import synth as SY
@@ -718,6 +889,9 @@ def census_step(variant):
     if variant == 'C2':
         cfg = SY.mv_det3d_config('C2')
         batch = SY.synth_batch(7, 1, n_views=20, H=480, W=640, n_points=100000, augment=True)
+    elif variant == 'C1':
+        cfg = SY.mv_det3d_config('C1')
+        batch = SY.synth_batch(1, 2, n_views=2, H=240, W=320, n_points=2000, augment=True)
     elif variant == 'C3':
         cfg = SY.mv_occ_config('C3')
         batch = SY.synth_batch(1, 1, n_views=2, H=240, W=320, n_points=4000)
@@ -730,7 +904,7 @@ def census_step(variant):
             SY.add_grounding_prompt(ds, 1 + 2 * i, seed=i)
     with warnings.catch_warnings():
         warnings.simplefilter('ignore')
-        model = MODELS.build(dict(cfg, compute_dtype=BF)).to(DEV).train()
+        model = MODELS.build(dict(cfg, compute_dtype=dtype)).to(DEV).train()
     return model, batch
 
 

@@ -1,7 +1,8 @@
-"""The head, loss and elementwise kernels of the bf16 training steps, pinned per element against a float64 reference on the
-same operands (tests/bf16_bounds.py) or bit for bit, and one census over the whole library: every library kernel a C2, C3
-or C4 bf16 training step (C2 with its optimiser step) launches is pinned here, in test_sparse_bf16_gpu.py or in
-test_dense_bf16_gpu.py, or is named in EXACT with the test that holds it bit for bit or to a fixture.
+"""The head, loss and elementwise kernels of the bf16 and fp32 training steps, pinned per element against a float64
+reference on the same operands (tests/bf16_bounds.py) or bit for bit, and one census over the whole library: every library
+kernel a C2, C3 or C4 bf16 training step (C2 with its optimiser step) or a C1 (with its optimiser step), C3 or C4 fp32
+training step launches is pinned here, in test_sparse_bf16_gpu.py or in test_dense_bf16_gpu.py, or is named in EXACT with
+the test that holds it bit for bit or to a fixture.
 
   * focal_fwd_kernel / focal_bwd_kernel (fp32 and bf16 logits): the loss sum and the per-element gradient against mmcv's
     formula in float64 (bf16_bounds.focal_ref, whose conditioning factor K(x) = 1 + e^|x| is part of the element term),
@@ -10,14 +11,14 @@ test_dense_bf16_gpu.py, or is named in EXACT with the test that holds it bit for
     checked on the smaller cases). Saturated logits (x <= -89, where expf overflows; x >= 17, where p rounds to 1) against
     mmcv's clamp to log(FLT_MIN) in closed form.
   * bias_act_kernel / act_bwd_kernel: the 2-D backbone's epilogue, in place as backbones._BiasResAct calls it.
-  * gather2_rows_kernel, img_normalize_kernel<bf16>, cast_kernel<bf16>: bit for bit.
+  * gather2_rows_kernel, img_normalize_kernel (bf16 and fp32), cast_kernel<bf16>: bit for bit.
   * interp_features_kernel: multilinear interpolation against float64 on the same features (an 11-term bound).
   * backbones._BiasResAct's bias gradient: a ResNet with a trainable BN affine in eval mode (norm_eval with the default
     norm_cfg) against a float64 restatement, fp32 and bf16, through the CUDA graph and without it.
 
 Worst ratios measured on an H100 SXM (80 GB HBM3, 132 SMs, 700 W power limit), c = C_ACC = 0.5 throughout: focal 0.0667,
 bias_act 0.284, act_bwd 0.367 (its `fixed` term carries the rest), interp 0.152; bf16_bounds.py's docstring has the
-details.
+details, and the fp32 ratios of the sparse and dense modules.
 
 Each case runs under torch.profiler in a fresh interpreter (head_elementwise_bf16_child.py) and claims the instances it
 launched, as the sparse and dense modules do."""
@@ -130,8 +131,9 @@ ACT_BWD = [f'act_bwd_kernel<{t}>' for t in ('float', '__nv_bfloat16')]
 GATHER2 = [f'gather2_rows_kernel<{t}>' for t in ('float', '__nv_bfloat16')]
 INTERP = [f'interp_features_kernel<{t}>' for t in ('float', '__nv_bfloat16')]
 IMG_NORM = 'img_normalize_kernel<__nv_bfloat16>'
+IMG_NORM_F32 = 'img_normalize_kernel<float>'
 CAST = 'cast_kernel<__nv_bfloat16>'
-PINNED = set(FOCAL) | set(BIAS_ACT) | set(ACT_BWD) | set(GATHER2) | set(INTERP) | {IMG_NORM, CAST}
+PINNED = set(FOCAL) | set(BIAS_ACT) | set(ACT_BWD) | set(GATHER2) | set(INTERP) | {IMG_NORM, IMG_NORM_F32, CAST}
 
 
 # ------------------------------------------------------------------------------------------------ focal loss
@@ -356,9 +358,10 @@ def test_interp_features(dtype, C, ts):
 # ------------------------------------------------------------------------------------------------ bit-exact elementwise
 @pytest.mark.parametrize('bgr', [0, 1])
 @pytest.mark.parametrize('channels_last', [0, 1])
-def test_img_normalize_bf16(channels_last, bgr):
-    """esb_img_normalize to bf16, bit for bit against CPU ((px - mean) / std) in fp32 then rounded to bf16 (the same
-    double rounding), on several images with H < Hp and W < Wp (the padding exactly zero), into NaN."""
+@pytest.mark.parametrize('dtype', [BF, F32], ids=['bf16', 'fp32'])
+def test_img_normalize(dtype, channels_last, bgr):
+    """esb_img_normalize to bf16 and fp32, bit for bit against CPU ((px - mean) / std) in fp32 (for bf16 then rounded to
+    bf16: the same double rounding), on several images with H < Hp and W < Wp (the padding exactly zero), into NaN."""
     from embodiedscan_b200._ffi import call, dtype_code, ptr, stream
     g = torch.Generator().manual_seed(channels_last * 2 + bgr)
     n, H, W, Hp, Wp = 3, 37, 45, 64, 64
@@ -366,15 +369,16 @@ def test_img_normalize_bf16(channels_last, bgr):
     mean, std = [123.675, 116.28, 103.53], [58.395, 57.12, 57.375]
     m3, s3 = (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std)
     shape = (n, Hp, Wp, 3) if channels_last else (n, 3, Hp, Wp)
-    dst = torch.full(shape, NAN, dtype=BF, device=DEV)
+    dst = torch.full(shape, NAN, dtype=dtype, device=DEV)
     sd = src.to(DEV)
     _, seen = _instances(lambda: call('esb_img_normalize', ptr(sd), n, H, W, Hp, Wp, ctypes.cast(m3, ctypes.c_void_p),
-                                      ctypes.cast(s3, ctypes.c_void_p), bgr, channels_last, ptr(dst), dtype_code(BF),
+                                      ctypes.cast(s3, ctypes.c_void_p), bgr, channels_last, ptr(dst), dtype_code(dtype),
                                       stream()))
-    _claim(seen, [IMG_NORM], f'img normalize cl {channels_last} bgr {bgr}')
+    _claim(seen, [IMG_NORM if dtype == BF else IMG_NORM_F32],
+           f'img normalize cl {channels_last} bgr {bgr}' + ('' if dtype == BF else ' fp32'))
     px = src.float()[:, [2, 1, 0]] if bgr else src.float()
-    v = ((px - torch.tensor(mean).view(1, 3, 1, 1)) / torch.tensor(std).view(1, 3, 1, 1)).float().to(BF)
-    ref = torch.zeros((n, 3, Hp, Wp), dtype=BF)
+    v = ((px - torch.tensor(mean).view(1, 3, 1, 1)) / torch.tensor(std).view(1, 3, 1, 1)).float().to(dtype)
+    ref = torch.zeros((n, 3, Hp, Wp), dtype=dtype)
     ref[:, :, :H, :W] = v
     got = dst.cpu().permute(0, 3, 1, 2) if channels_last else dst.cpu()
     assert torch.equal(got, ref)
@@ -543,7 +547,7 @@ EXACT = {
 def _pinned_everywhere():
     import test_dense_bf16_gpu as D
     import test_sparse_bf16_gpu as S
-    return S.PINNED | D.PINNED | PINNED
+    return S.PINNED | S.PINNED_F32 | D.PINNED | D.PINNED_F32 | PINNED
 
 
 def unheld(seen, pinned, exact):
@@ -565,36 +569,51 @@ def test_exact_table_names_existing_tests():
 test_exact_table_names_existing_tests.no_child = True
 
 
-@pytest.mark.parametrize('variant', ['C2', 'C3', 'C4'])
+# the census steps: bf16 C2 (with its optimiser step), C3, C4; fp32 (the parity arithmetic) C1 (with its optimiser step),
+# C3, C4
+CENSUS = ['C2', 'C3', 'C4', 'C1-fp32', 'C3-fp32', 'C4-fp32']
+
+
+def _census_label(variant):
+    name, _, dt = variant.partition('-')
+    return f'{name} {dt or "bf16"} step, whole library'
+
+
+@pytest.mark.parametrize('variant', CENSUS)
 def test_step_launches_only_held_library_kernels(variant):
-    """One bf16 training forward + backward of C2 (with the OptimWrapper step: cast, clip and AdamW), C3 and C4 on the
-    census batches of test_dense_bf16_gpu.py: every library kernel instance launched must be pinned (here, or in the
-    sparse or dense module) or, by kernel name, held bit for bit or to a fixture by the test EXACT names."""
+    """One training forward + backward of C2 (with the OptimWrapper step: cast, clip and AdamW), C3 and C4 in bf16, and of
+    C1 (with its OptimWrapper step), C3 and C4 in fp32, on the census batches of test_dense_bf16_gpu.py: every library
+    kernel instance launched must be pinned (here, or in the sparse or dense module) or, by kernel name, held bit for bit
+    or to a fixture by the test EXACT names."""
+    name, _, dt = variant.partition('-')
+    with_optim = name in ('C1', 'C2')
     if _CHILD is None:
-        seen = _claim(set(), [], f'{variant} bf16 step, whole library')
+        seen = _claim(set(), [], _census_label(variant))
     else:
         import test_dense_bf16_gpu as D
         from embodiedscan_b200.engine import OptimWrapper
-        model, batch = D.census_step(variant)
-        optim = OptimWrapper(model) if variant == 'C2' else None
+        model, batch = D.census_step(name, F32 if dt == 'fp32' else BF)
+        optim = OptimWrapper(model) if with_optim else None
 
         def step():
             data = model.data_preprocessor(dict(inputs=batch['inputs'], data_samples=batch['data_samples']), True)
             loss = sum(model(**data, mode='loss').values())
             optim.update_params(loss) if optim is not None else loss.backward()
-        seen = _claim(_instances(step)[1], [], f'{variant} bf16 step, whole library')
+        seen = _claim(_instances(step)[1], [], _census_label(variant))
     assert len(seen) > 20, f'the profiler saw only {sorted(seen)}'
     if variant == 'C2':
         assert CAST in seen, 'the optimiser step was not recorded'
+    if with_optim:
+        assert any(i.split('<')[0] == 'adamw_kernel' for i in seen), 'the optimiser step was not recorded'
     bad = unheld(seen, _pinned_everywhere(), EXACT)
     assert not bad, f'library kernels no test holds: {bad}'
 
 
 def test_census_rule_names_what_it_misses():
     """Dropping any one entry of the pinned sets or of EXACT makes the rule fail with that kernel's name, on the
-    instances the census steps launched."""
+    instances the bf16 and fp32 census steps launched."""
     rec = _launched()
-    seen = set().union(*(rec.get(f'{v} bf16 step, whole library', ()) for v in ('C2', 'C3', 'C4')))
+    seen = set().union(*(rec.get(_census_label(v), ()) for v in CENSUS))
     pinned = _pinned_everywhere()
     assert not unheld(seen, pinned, EXACT)
     for inst in sorted(seen & pinned):
