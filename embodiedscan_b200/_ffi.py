@@ -76,6 +76,7 @@ SIGNATURES = {
     'esb_nms3d_9dof': ('pppp' + 'ii' + 'ff' + 'ii' + 'ppp' + 'zp', 'i'),
     'esb_hungarian_batch': ('ppiiippp', 'i'),
     'esb_img_normalize': ('piiiiippiipip', 'i'),
+    'esb_img_resize_linear_u8': ('piiiiipp', 'i'),
     'esb_unproject_depth_workspace_bytes': ('iii', 'z'),
     'esb_unproject_depth': ('piiifpppppzp', 'i'),
     'esb_grad_clip_coef': ('pqffpp', 'i'),

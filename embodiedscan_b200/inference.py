@@ -13,7 +13,7 @@ import torch
 from .detectors import Embodied3DDetector, SparseFeatureFusionSingleStage3DDetector
 from .geometry import nms3d_9dof
 from .structures import Det3DDataSample, EulerDepthInstance3DBoxes, InstanceData
-from .transforms import MultiViewDepthToPoints
+from .transforms import MultiViewDepthToPoints, MultiViewResize
 
 # camera axes (x right, y down, z forward) -> the pose file's body axes (demo.py:180-181)
 _CAM_AXES = np.array([[0., 0., 1.], [-1., 0., 0.], [0., -1., 0.]])
@@ -72,7 +72,7 @@ def _intrinsic44(intrinsic) -> np.ndarray:
 
 
 def inference_scan(model, imgs_u8: torch.Tensor, depth_u16: torch.Tensor, intrinsic, extrinsics, *, num_points: int,
-                   points_per_view: int, depth_shift: float = 1000., seed: int = 0, filter=None):
+                   points_per_view: int, depth_shift: float = 1000., seed: int = 0, filter=None, img_scale=None):
     """One posed RGB-D scan through a detector and the final box filter.
 
     imgs_u8 (V,H,W,3) uint8 colour frames in the channel order the model's preprocessor expects, depth_u16 (V,H,W)
@@ -82,7 +82,13 @@ def inference_scan(model, imgs_u8: torch.Tensor, depth_u16: torch.Tensor, intrin
     Returns ``(results, filtered)``: `results` is the list of ``Det3DDataSample`` of ``model.forward(mode='predict')``
     with ``pred_instances_3d`` set, one for ``SparseFeatureFusionSingleStage3DDetector`` and one per frame prefix
     1..V for ``Embodied3DDetector``; `filtered[i]` is ``nms_filter(results[i].pred_instances_3d)``, all results
-    filtered in one launch. Points are sampled as ``MultiViewDepthToPoints`` samples them, seeded by `seed`."""
+    filtered in one launch. Points are sampled as ``MultiViewDepthToPoints`` samples them, seeded by `seed`.
+
+    `img_scale` ``(w, h)`` resizes the colour frames as the config's ``Resize(scale=(w, h), keep_ratio=False)`` does
+    (``MultiViewResize``, cv2 bilinear bit for bit) and records its ``img_shape`` and ``scale_factor``, so point
+    painting maps the intrinsics of the original frames onto the resized ones. The config's ``Resize`` scale (480x480 in
+    every published config) is what reproduces ``demo.py``, which runs the config's test pipeline. ``None`` passes the
+    frames at their own size, as a pipeline without ``Resize`` would."""
     if not isinstance(model, SparseFeatureFusionSingleStage3DDetector):
         raise TypeError(f'inference_scan runs the box detectors (SparseFeatureFusionSingleStage3DDetector, '
                         f'Embodied3DDetector); {type(model).__name__} predicts no boxes (occupancy and grounding models '
@@ -93,10 +99,15 @@ def inference_scan(model, imgs_u8: torch.Tensor, depth_u16: torch.Tensor, intrin
     V, H, W = depth_u16.shape
     assert imgs_u8.dtype == torch.uint8 and tuple(imgs_u8.shape) == (V, H, W, 3) and len(extrinsics) == V
     depth = depth_u16.to(dev)
-    img = imgs_u8.to(dev).permute(0, 3, 1, 2).contiguous()                   # (V,3,H,W) uint8, as Pack3DDetInputs
+    if img_scale is None:
+        img = imgs_u8.to(dev).permute(0, 3, 1, 2).contiguous()               # (V,3,H,W) uint8, as Pack3DDetInputs
+        img_shape, scale_factor = (H, W), (1.0, 1.0)
+    else:
+        resized = MultiViewResize(img_scale)(dict(img=imgs_u8.to(dev)))
+        img, img_shape, scale_factor = resized['img'], resized['img_shape'], resized['scale_factor']
     K = _intrinsic44(intrinsic)
     extr = [np.asarray(e, dtype=np.float32).reshape(4, 4) for e in extrinsics]
-    meta = dict(img_shape=(H, W), ori_shape=(H, W), scale_factor=(1.0, 1.0), flip=False, transformation_3d_flow=[],
+    meta = dict(img_shape=img_shape, ori_shape=(H, W), scale_factor=scale_factor, flip=False, transformation_3d_flow=[],
                 depth2img=dict(extrinsic=extr, intrinsic=[K] * V, origin=np.array([.0, .0, .5], dtype=np.float32)),
                 box_type_3d=EulerDepthInstance3DBoxes)
     sample = Det3DDataSample(metainfo=meta)

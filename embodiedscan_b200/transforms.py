@@ -2,6 +2,8 @@
 launch, replacing LoadDepthFromFile's `/ depth_shift`, ConvertRGBDToPoints + points_img2cam and AggregateMultiViewPoints
 (embodiedscan/datasets/transforms/loading.py:70-73, points.py:30-81, structures/bbox_3d/utils.py:335-368,
 multiview.py:139-169), followed by the reference's two PointSample stages (points.py:119-153) as seeded permutations.
+The colour frames' `Resize` of the same pipeline (cv2 bilinear, bit for bit) is `MultiViewResize`, all views in one
+launch.
 
 The 3D augmentations of the training pipeline (configs/detection/mv-det3d_*.py:147-158) follow as torch operations on
 the device-resident points and the (tiny) box tensor: `RandomFlip3D` (datasets/transforms/augmentation.py:11-250, the
@@ -73,6 +75,53 @@ class MultiViewDepthToPoints:
         keep = keep[torch.randperm(keep.numel(), generator=gen, device=pts.device)[:self.num_points]]
         results['points'] = pts[keep].contiguous()
         return results
+
+
+def resize_multiview(img_u8: torch.Tensor, size) -> torch.Tensor:
+    """(V,H,W,3) uint8 frames on the GPU -> (V,3,h,w) uint8 for ``size = (w, h)``: ``cv2.resize(frame, size,
+    interpolation=cv2.INTER_LINEAR)`` of every view, bit for bit, in one launch (csrc/resize.cu). Channels keep their
+    order; the output is the layout ``Pack3DDetInputs`` stacks."""
+    assert isinstance(img_u8, torch.Tensor) and img_u8.is_cuda and img_u8.dtype == torch.uint8 and \
+        img_u8.dim() == 4 and img_u8.shape[-1] == 3, 'frames are one (V,H,W,3) uint8 GPU tensor (one source size)'
+    w, h = (int(s) for s in size)
+    V, H, W, _ = img_u8.shape
+    src = img_u8.contiguous()
+    out = torch.empty((V, 3, h, w), dtype=torch.uint8, device=src.device)
+    call('esb_img_resize_linear_u8', ptr(src), V, H, W, h, w, ptr(out), stream())
+    return out
+
+
+@TRANSFORMS.register_module()
+class MultiViewResize:
+    """mmcv's ``Resize(scale=(w, h), keep_ratio=False)`` as the configs run it inside ``MultiViewPipeline``
+    (configs/detection/mv-det3d_*.py:143,171), for all views of a scan at once: results['img'] (V,H,W,3) uint8 on the
+    GPU -> (V,3,h,w). It leaves the keys mmcv's ``Resize._resize_img`` writes for the last view, which
+    ``MultiViewPipeline`` keeps (multiview.py:90-92): ``img_shape = (h, w)``, ``scale = (w, h)``,
+    ``scale_factor = (w / W, h / H)`` and ``keep_ratio``. Point painting reads ``scale_factor`` to map the original
+    intrinsics onto the resized pixels (fusion.py). Only the configured mode is implemented: a fixed size, bilinear
+    (mmcv's default cv2 backend)."""
+
+    def __init__(self, scale, keep_ratio: bool = False, interpolation: str = 'bilinear'):
+        if keep_ratio:
+            raise ValueError('MultiViewResize: keep_ratio=True is not on the configured path (the configs resize to a '
+                             'fixed size)')
+        if interpolation != 'bilinear':
+            raise ValueError(f'MultiViewResize: only bilinear interpolation is implemented, got {interpolation!r}')
+        self.scale = (scale, scale) if isinstance(scale, int) else tuple(scale)
+        self.keep_ratio = keep_ratio
+
+    def __call__(self, results: dict) -> dict:
+        img = results['img']
+        results['img'] = resize_multiview(img, self.scale)
+        H, W = img.shape[1:3]
+        w, h = self.scale
+        results['img_shape'] = (h, w)
+        results['scale'] = self.scale
+        results['scale_factor'] = (w / W, h / H)
+        results['keep_ratio'] = self.keep_ratio
+        return results
+
+    transform = __call__
 
 
 @TRANSFORMS.register_module()

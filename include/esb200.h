@@ -264,6 +264,12 @@ int esb_hungarian_batch(const float* cost, const int* n_gt, int n_problems, int 
  * depth->points unprojection (datasets/transforms/points.py:30-81, multiview.py:139-169) ------------------------- */
 int esb_img_normalize(const unsigned char* src, int n_img, int H, int W, int Hp, int Wp, const float* mean3_host,
                       const float* std3_host, int bgr_to_rgb, int channels_last, void* dst, int dtype, void* stream);
+/* MultiViewPipeline's `Resize(scale=(w, h), keep_ratio=False)` (cv2.resize INTER_LINEAR through mmcv imresize, bit for
+ * bit, including cv2's switch to INTER_AREA at an exact 2x downscale on both axes and its copy at an unchanged size):
+ * src (V,H,W,3) uint8 as decoded -> dst (V,3,h,w) uint8, channel order unchanged. One launch for all V views
+ * (V <= 65535). */
+int esb_img_resize_linear_u8(const unsigned char* src, int V, int H, int W, int h, int w, unsigned char* dst,
+                             void* stream);
 size_t esb_unproject_depth_workspace_bytes(int V, int H, int W);
 int esb_unproject_depth(const unsigned short* depth, int V, int H, int W, float depth_shift, const float* mats,
                         float* out, int* view_of, int* count_dev, void* ws, size_t ws_bytes, void* stream);
